@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — VampNet masked-token generation hot path on B200 (contract in the task statement).
+"""bench.py — VampNet masked-token generation hot path on the H100 (sm_90a); prints one JSON result line.
 
     python bench.py --gpus N --steps K --warmup W [--config {1,2,3,4}]     # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K --warmup W         # CPU arm (oracle port of the reference)
     torchrun ... bench.py --gpus N ...                                     # N>1: one rank per GPU, weak scaling
+    python bench.py ... --dump-outputs DIR                                 # also save the last timed step's output
 
 --config selects BASELINE.json configs[k] (default 2, the configuration the metric "coarse+c2f" is quoted on):
   1  coarse generate: 12 sampling steps, T=768, B=8 per GPU
@@ -15,6 +16,11 @@ One "step" = one pass of that workload over one batch of synthetic input (random
 synthetic audio, periodic prompt every 7th frame, default sampling parameters: temperature 1, mask_temperature 10.5).
 value = codec tokens/s = N*B*T*C_out / time (C_out = 4 for the coarse-only configs, 14 otherwise); real-time factor
 = N*B*T*768/44100 / time.
+--dump-outputs DIR writes what the last timed step returned (rank 0) as DIR/tokens.npy (float32 token ids, configs 1, 2,
+4) or DIR/audio.npy (float32 samples, config 3).  An output above 64 MB is written as a fixed seeded sample instead:
+DIR/<name>_sample.npy (4 Mi float32 values) and DIR/<name>_sample_index.npy (their float64 flat indices), 48 MB
+together.  Weights, codes and audio are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -55,6 +61,10 @@ CONFIGS = {
             workload="BASELINE.json configs[4]: coarse generate 24 steps, T=3072 (~40 s), d=1280, 20 layers"),
 }
 MODEL_CFG = {"coarse": COARSE, "c2f": C2F}
+# NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16 tensor throughput.  Shares of peak below are
+# relative to these; a card at a lower power limit, or clocking down under load, reaches less.
+H100_HBM_GBS, H100_BF16_TFLOPS = 3350.0, 989.0
+DUMP_MAX_BYTES = 64 << 20  # --dump-outputs writes at most this much
 # codec algorithmic work per 10 s clip (SURVEY.md section 8d, stand-in configuration): fp32 layer-by-layer bytes, flops
 CODEC_BYTES = {"encode": 8.3e9, "decode": 12.4e9}
 CODEC_FLOPS = {"encode": 0.61e12, "decode": 1.37e12}
@@ -88,33 +98,6 @@ def gemm_algorithmic_bytes(B, T, d=1280):
     up = M * d * 2 + 4 * d * d * 2 + M * 2 * d * 2
     down = M * 2 * d * 2 + 2 * d * d * 2 + M * d * (4 + 4 + 2)
     return (qkv + out + up + down) / 4.0
-
-
-def ncu_traffic_per_launch():
-    """dram__bytes_read.sum + dram__bytes_write.sum per GEMM launch from the committed `ncu --set full` summary
-    (profiles/ncu_layer_r2.txt: one layer's qkv / attn-out / ffn-up / ffn-down at the bench shape)."""
-    name = next((n for n in ("ncu_layer_r2.txt", "ncu_gemm_r1_pair.txt", "ncu_gemm_r1_final.txt")
-                 if os.path.exists(os.path.join(ROOT, "profiles", n))), "ncu_layer_r2.txt")
-    path = os.path.join(ROOT, "profiles", name)
-    try:
-        per_kind, cur = {}, None
-        for line in open(path):
-            if line.startswith("== "):
-                cur = line.split("gemm_tcgen05_kernel<")[1][0] if "gemm_tcgen05_kernel<" in line else None
-                if cur is not None:
-                    per_kind.setdefault(cur, []).append(0.0)
-            elif cur is not None and ("dram__bytes_read.sum " in line or "dram__bytes_write.sum " in line):
-                f = line.split()
-                val, unit = float(f[1]), f[2].lower()
-                per_kind[cur][-1] += val * {"byte": 1.0, "kbyte": 1e3, "mbyte": 1e6, "gbyte": 1e9}[unit]
-        # <1> qkv, <2> residual epilogue (attn-out and ffn-down alternate), <3> ffn-up: weight 1 : 2 : 1
-        if not all(k in per_kind for k in "123"):
-            return None, f"profiles/{name} incomplete"
-        mean = lambda v: sum(v) / len(v)
-        return (mean(per_kind["1"]) + 2 * mean(per_kind["2"]) + mean(per_kind["3"])) / 4.0, \
-            f"profiles/{name} (ncu --set full, B=32 T=768 coarse layer)"
-    except Exception as e:  # the summary is evidence, not a dependency
-        return None, f"unavailable: {e}"
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -292,11 +275,10 @@ def emit(line: dict):
     os.write(_REAL_STDOUT if _REAL_STDOUT is not None else 1, data)
 
 
-def secondary_rooflines(cfg, B, fam_ms, fam_n, fl, peaks, codec_ms):
+def secondary_rooflines(cfg, B, fam_ms, fam_n, fl, codec_ms):
     """The kernels the north-star classifies by HBM bandwidth, and attention by tensor throughput, next to the headline
     GEMM family: achieved = ALGORITHMIC bytes (or flops) of the launches of one profiled step / their CUDA-event time."""
-    hbm = peaks.get("hbm_gbs", 6650.0)
-    tf = peaks.get("bf16_tflops_sustained", 1400.0)
+    hbm, tf = H100_HBM_GBS, H100_BF16_TFLOPS
     out = []
     T = cfg["T"]
     logit_bytes = emb_bytes = 0.0
@@ -333,16 +315,16 @@ def secondary_rooflines(cfg, B, fam_ms, fam_n, fl, peaks, codec_ms):
                     "frac": a / hbm, "algorithmic_bytes_per_step": emb_bytes, "ms_per_step": fam_ms["embed"]})
     if fam_ms.get("attention"):
         a = fl["attention"] / (fam_ms["attention"] * 1e-3) / 1e12
-        out.append({"kernel": "attention_tcgen05_kernel", "bound": "tensor", "achieved": a, "peak": tf, "unit": "TFLOP/s",
+        out.append({"kernel": "attention_wgmma_kernel", "bound": "tensor", "achieved": a, "peak": tf, "unit": "TFLOP/s",
                     "frac": a / tf, "ms_per_step": fam_ms["attention"],
-                    "note": "at d_head 64 the exponentials (MUFU) cost twice the tensor cycles: MUFU-bound ceiling = 0.5"})
+                    "note": "FlashAttention-style: S and P in registers, two consumer warpgroups per 128 queries"})
     for part in ("encode", "decode"):
         if codec_ms.get(part):
             t = codec_ms[part] * 1e-3
             ab, af = B * CODEC_BYTES[part] / t / 1e9, B * CODEC_FLOPS[part] / t / 1e12
-            out.append({"kernel": f"codec {part} (conv_tcgen05_kernel stack + rvq_kernel)", "bound": "hbm",
+            out.append({"kernel": f"codec {part} (conv_wgmma_kernel stack + rvq_kernel)", "bound": "hbm",
                         "achieved": ab, "peak": hbm, "unit": "GB/s", "frac": ab / hbm, "ms_per_step": codec_ms[part],
-                        "tflops": af, "tensor_frac_of_sustained_bf16": af / tf,
+                        "tflops": af, "tensor_frac_of_bf16_peak": af / tf,
                         "note": "bytes = fp32 layer-by-layer activation traffic of the stand-in architecture (SURVEY.md 8d); "
                                 "split-bf16 issues 3 MMAs per algorithmic one"})
     return out
@@ -358,6 +340,8 @@ def main():
     ap.add_argument("--config", type=int, default=2, choices=sorted(CONFIGS), help="BASELINE.json configs[k]")
     ap.add_argument("--batch", type=int, default=None, help="clips per GPU (default = the named config)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -503,6 +487,19 @@ def main():
     ms = e0.elapsed_time(e1)
     launches = lib.vnb_launch_count() - launches0
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        name = "audio" if cfg["codec"] else "tokens"
+        arr = out.float().cpu().numpy()
+        if arr.nbytes > DUMP_MAX_BYTES:
+            # fixed seeded sample of the flat output (same entries in every run with the same shape) + their indices
+            n = DUMP_MAX_BYTES // 16
+            idx = torch.randperm(arr.size, generator=torch.Generator().manual_seed(0))[:n].sort().values.numpy()
+            np.save(os.path.join(args.dump_outputs, f"{name}_sample_index.npy"), idx.astype(np.float64))
+            arr = arr.reshape(-1)[idx]
+            name += "_sample"
+        np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
 
     # ---- end to end: host (pinned) inputs, H2D + D2H inside the timed region, public API ----
     barrier()
@@ -546,28 +543,19 @@ def main():
     gemm_ms = sum(fam_ms[k] for k in gemm_keys)
     gemm_fl = sum(fl[k] for k in gemm_keys)
     gemm_n = sum(fam_n[k] for k in gemm_keys)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)  # kernel timed inside a long step -> sustained figure
-    traffic, traffic_note = ncu_traffic_per_launch()
-    if (B, T) != (32, 768):
-        traffic, traffic_note = None, "the committed ncu capture is of the B=32, T=768 shape"
+    peak_tf = H100_BF16_TFLOPS
     achieved = gemm_fl / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
     roofline = {
-        "kernel": "gemm_tcgen05_kernel<EPI, PAIR=true> (CTA pairs, tcgen05.mma.cta_group::2, 256x256 tiles; all epilogues: qkv, attn-out+residual, ffn-up+GEGLU, ffn-down+residual, classifier+bias)",
+        "kernel": "gemm_wgmma_kernel<EPI, PAIR> (128x256 tiles, wgmma m64n256k16, TMA 4-stage ring; PAIR per option gemm_pair, default single CTA; all epilogues: qkv, attn-out+residual, ffn-up+GEGLU, ffn-down+residual, classifier+bias)",
         "bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-        "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained",
-        "traffic": traffic, "traffic_unit": "bytes per launch (dram read+write)", "traffic_source": traffic_note,
+        "peak_source": "H100 SXM data sheet, dense BF16",
         "algorithmic_bytes_per_launch": gemm_algorithmic_bytes(B, T),
         "flops_per_launch": gemm_fl / max(gemm_n, 1), "avg_launch_us": 1e3 * gemm_ms / max(gemm_n, 1),
         "share_of_step": gemm_ms / prof_total if prof_total else None,
         "breakdown_ms": {**{k: round(fam_ms[k], 3) for k in _lib.FAMILIES}, **{"codec_" + k: round(v, 3) for k, v in codec_ms.items()}},
         "breakdown_tflops": {k: (fl[k] / (fam_ms[k] * 1e-3) / 1e12 if fam_ms.get(k) else None) for k in fl},
         "profiled_step_ms": prof_total,
-        "secondary": secondary_rooflines(cfg, B, fam_ms, fam_n, fl, peaks, codec_ms),
+        "secondary": secondary_rooflines(cfg, B, fam_ms, fam_n, fl, codec_ms),
     }
 
     if rank == 0:
@@ -584,7 +572,7 @@ def main():
             "tflops": world * flops_step * args.steps / (ms * 1e-3) / 1e12,
             "config": {"workload": cfg["workload"], "baseline_config_index": args.config,
                        "global_batch": world * B, "per_gpu_batch": B, "seq_len": T, "parallelism": f"dp{world} (clips)",
-                       "l2": "working set per step (1.3-2.4 GB of bf16 weights, plus ~1 GB of activations per layer) far exceeds the 126 MB L2",
+                       "l2": "working set per step (1.3-2.4 GB of bf16 weights, plus ~1 GB of activations per layer) far exceeds the 50 MB L2",
                        "weights": "random-init, NCCL-broadcast from rank 0", "cuda_graph": True},
             "clocks": clk,
             "e2e": {"value": tokens / (e2e_ms * 1e-3), "unit": "tokens/s", "h2d_bytes_per_step": h2d * world,

@@ -1,4 +1,4 @@
-/* vampnet_b200 — C ABI of the B200-native VampNet masked-token generation hot path.
+/* vampnet_b200 — C ABI of the H100-native (sm_90a) VampNet masked-token generation hot path.
  *
  * The reference (hugofloresgarcia/vampnet) is pure Python/PyTorch and has no FFI of its own; its
  * boundary is the Python class surface (SURVEY.md §8b).  These entry points are what a binding
@@ -127,14 +127,15 @@ uint64_t vnb_launch_count(void);
 uint64_t vnb_graph_capture_count(void);
 
 /* ---- tuning options ----------------------------------------------------------------------------
- * "gemm_pair": 1 = dense contractions run as CTA pairs (tcgen05.mma.cta_group::2, 256 x 256 tiles, each SM stages
- *              half of the weight tile), 0 = one CTA per 128 x 256 tile.  Results are bit-identical (same
+ * "gemm_pair": 1 = dense contractions run as clusters of two CTAs on vertically adjacent 128 x 256 tiles that share
+ *              the weight tile (each CTA fetches half of it, TMA multicast), 0 (default, faster on H100) = one CTA
+ *              per 128 x 256 tile.  Results are bit-identical (same
  *              accumulation order per output element).  Initial value: environment VNB_GEMM_PAIR, else the
  *              compiled default.  Generate graphs are cached per value.
  * "fused_sampler": 1 (default) = vnb_generate samples inside the classifier GEMM's epilogue (VNB_EPI_SAMPLE: the logits of
  *   the generate loop never reach HBM), 0 = from a materialised fp32 logits tensor (sample_rows_kernel).  Both draw
  *   with the same two-level inverse CDF and the same Philox stream; nucleus (top-p) sampling always materialises.
- * "gemm_pair_max_clusters" (get only): CTA pairs that can be co-resident on the current device. */
+ * "gemm_pair_max_clusters" (get only): clusters of two that can be co-resident on the current device. */
 int32_t vnb_set_option(const char* name, int32_t value);
 int32_t vnb_get_option(const char* name, int32_t* value);
 int32_t vnb_profile_begin(vnb_model* m);
@@ -150,7 +151,7 @@ enum {
   VNB_EPI_SAMPLE = 5    /* internal to vnb_generate: acc + bias[n] sampled per 128-column strip, nothing stored but
                            16 bytes per (row, strip); not accepted by vnb_op_gemm */
 };
-/* out = A (M,K) bf16 row-major  x  W (N,K)^T bf16 row-major, fp32 accumulate in TMEM.
+/* out = A (M,K) bf16 row-major  x  W (N,K)^T bf16 row-major, fp32 accumulation (wgmma).
  * N % 256 == 0, K % 64 == 0.  For VNB_EPI_QKV: out = qk, out2 = vT, T/Tpad describe the batch split. */
 int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
                     void* out2, const float* bias, int32_t T, int32_t Tpad, void* stream);
@@ -158,7 +159,7 @@ int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_
  * qk (B, T, 2d) bf16 [q | k], vT (B, d, Tpad) bf16, out (B, T, d) bf16, d = H*64. */
 int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                          int32_t B, int32_t T, int32_t Tpad, int32_t H, void* stream);
-/* Naive SIMT GEMM used only to bisect the tcgen05 path in tests: out fp32 (M, N) = A x W^T. */
+/* Naive SIMT GEMM used only to bisect the tensor-core path in tests: out fp32 (M, N) = A x W^T. */
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream);
 
 /* ---- codec (DAC family; reference call sites: interface.py:223 codec.encode, transformer.py:671-675
@@ -179,7 +180,7 @@ int32_t vnb_codec_rvq(int32_t mode, const float* in_f, const int64_t* in_codes, 
                       const float* wout, const float* bout, const float* cb, const float* cbn, int64_t* codes, float* zq,
                       float* latents, int32_t B, int32_t D, int32_t T, int32_t L, int32_t V, int32_t channels_last,
                       void* zq_hi, void* zq_lo, void* stream);
-/* Tensor-core codec path (tcgen05, split-bf16 operands = fp32-grade products; see csrc/conv_tcgen05.cu).
+/* Tensor-core codec path (wgmma, split-bf16 operands = fp32-grade products; see csrc/conv_wgmma.cu).
  * Activations are channels-last (B, T, C) and travel as hi/lo bf16 pairs (x = hi + lo).
  *   y[b, q, n] = bias[n % bias_mod] + sum_tap sum_ci W[n, tap, ci] * a[b, q*s + tap*dil - pad, ci]   (+ resid)
  * w_hi/w_lo: (N, taps * ceil(Cin/64) * 64) bf16, tap-major, channel blocks zero-padded to 64.

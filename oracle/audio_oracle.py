@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — independent CPU restatement of the audio preprocessing either side of the hot path
 (reference interface.py:206-217: resample -> mono -> normalize(-24 LUFS) -> ensure_max_of_audio; app.py:175-178, 247-248).
 
-The reference delegates this to ``descript-audiotools`` (third-party, unpinned, absent from /root/reference and from the
+The reference delegates this to ``descript-audiotools`` (third-party, unpinned, absent from the original project's checkout and from the
 image: PARITY UNPINNED against it).  What can be pinned is the published standard the library implements:
 
   * loudness: ITU-R BS.1770-4 integrated loudness — the two K-weighting biquads with the coefficients TABULATED IN THE

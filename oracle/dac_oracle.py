@@ -2,7 +2,7 @@
 
 The reference's codec is ``lac.model.lac.LAC`` (``lac @ git+https://github.com/hugofloresgarcia/lac.git``,
 unpinned git HEAD, reference requirements.txt:6 / setup.py:31), a Descript-Audio-Codec fork that is NOT under
-/root/reference and not installed here.  Its arithmetic is therefore restated from the published DAC
+the original project's checkout and not installed here.  Its arithmetic is therefore restated from the published DAC
 architecture as implemented by the in-image ``transformers.models.dac.modeling_dac`` (same family; line
 numbers below refer to that file), and anchored on the reference's own call sites:
   codec.preprocess / codec.encode(...)["codes"]          interface.py:215, 223

@@ -1,13 +1,12 @@
 """TEST INFRASTRUCTURE — not product code.
 
-Import the *unmodified* reference modules from /root/reference through two tiny
-shims, so that the reference's own code can be executed as the ground truth
-when golden vectors are generated (oracle/gen_golden.py) and when the CPU
-restatement (oracle/vampnet_oracle.py) is pinned (tests/test_oracle_vs_reference.py).
+Import the *unmodified* reference modules from a checkout of the original project
+($VAMPNET_REFERENCE_ROOT) through two tiny shims, so that the reference's own code can
+be executed as the ground truth when golden vectors are generated (oracle/gen_golden.py,
+oracle/gen_reference_golden.py).  The tests use only the stored vectors.
 
-Nothing is copied: the reference files are imported from where they lie.
-/root/reference exists only in the authoring container, never on the GPU box,
-so everything here is optional at run time (``available()`` says whether it is).
+Nothing is copied: the reference files are imported from where they lie
+(``available()`` says whether a checkout is there).
 
 Shims (SURVEY.md §8c):
   * ``audiotools``  -> ml.BaseModel = nn.Module subclass with a .device
@@ -17,7 +16,7 @@ Shims (SURVEY.md §8c):
     (loralib semantics, lora_alpha=1 default => scaling = 1/r) so that LoRA
     folding in the product can be checked against an unfused evaluation.
   * the reference package itself is imported under the name ``vampnet_reference``: a synthetic
-    package object whose __path__ points at /root/reference/vampnet, so vampnet/__init__.py (HF hub +
+    package object whose __path__ points at the checkout's vampnet/, so vampnet/__init__.py (HF hub +
     lac + librosa imports) is skipped and the name ``vampnet`` stays free for this repository's own
     drop-in package (vampnet/ at the repo root).  The reference only uses relative imports inside
     its package, so the name it is imported under does not matter.
@@ -35,7 +34,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-REFERENCE_ROOT = os.environ.get("VAMPNET_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VAMPNET_REFERENCE_ROOT", "")
 PKG = "vampnet_reference"
 
 

@@ -326,7 +326,7 @@ class OracleVampNet:
         else:
             # the CUDA sampler's draw (same distribution as multinomial): a two-level inverse CDF in natural
             # vocabulary order.  The vocabulary is cut into tiles of 128 entries (what one epilogue thread of the
-            # classifier GEMM holds, csrc/gemm_tcgen05.cu EPI_SAMPLE); uniform 1 picks the tile by its probability
+            # classifier GEMM holds, csrc/gemm_wgmma.cu EPI_SAMPLE); uniform 1 picks the tile by its probability
             # mass, uniform 2 the entry inside it: token = first v in the tile with cumsum(e)[v] > u2 * mass(tile).
             u1 = philox.uniform_bs(philox_key, step, B, S, stream=0, word=0)  # (B, S) fp32 in (0,1)
             u2 = philox.uniform_bs(philox_key, step, B, S, stream=0, word=1)

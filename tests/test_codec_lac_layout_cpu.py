@@ -1,7 +1,7 @@
 """CPU: the codec ingests checkpoints written in the descript-audio-codec / ``lac`` module layout — the layout of the
 file the reference's Interface actually loads (``lac.model.lac.LAC``, reference interface.py:16, 70).
 
-``lac`` itself is absent from /root/reference and from the image, so the module tree below is a TEST-LOCAL
+``lac`` itself is absent from the original project's checkout and from the image, so the module tree below is a TEST-LOCAL
 restatement of the published DAC module structure (nn.Sequential stacks of weight-normed convs and Snake1d with a
 (1, C, 1) alpha).  It is built with torch's own ``nn.Sequential`` / ``weight_norm`` so that the state_dict KEY NAMES
 are produced by torch, not typed by hand, and its forward pass (plain torch, CPU) pins the remapped weights

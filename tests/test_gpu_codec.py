@@ -10,7 +10,7 @@ from oracle import dac_oracle as do
 pytestmark = pytest.mark.gpu
 
 
-PRECISIONS = ["tc", "fp32"]  # tcgen05 split-bf16 convolutions (default) and the fp32 CUDA-core kernels
+PRECISIONS = ["tc", "fp32"]  # wgmma split-bf16 convolutions (default) and the fp32 CUDA-core kernels
 
 
 def build(cfg, seed=0, precision="tc"):

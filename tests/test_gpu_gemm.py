@@ -1,6 +1,7 @@
-"""GPU: the tcgen05 GEMM family through the C ABI (vnb_op_gemm) against an fp32 torch contraction of the same bf16
+"""GPU: the wgmma GEMM family through the C ABI (vnb_op_gemm) against an fp32 torch contraction of the same bf16
 operands, for every fused epilogue, ragged M, more tiles than SMs, and BOTH tile variants: one CTA per 128 x 256 tile
-and the CTA pair (tcgen05.mma.cta_group::2, 256 x 256 tiles; vnb_set_option "gemm_pair").  Tolerances: outputs are
+and the CTA pair (a cluster of two vertically adjacent tiles sharing the W tile by TMA multicast; vnb_set_option
+"gemm_pair").  Tolerances: outputs are
 bf16-rounded (rel 2^-8) or fp32 of a bf16 x bf16 -> fp32 accumulation; the two variants must agree bit for bit."""
 import math
 

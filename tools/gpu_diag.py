@@ -1,6 +1,6 @@
 """Development diagnostic (not a test, not product): run ONE kernel family on the GPU and print error
-statistics against a plain torch computation.  Each stage runs in its own process (tools/gpu_diag.sh)
-so that a trapping kernel cannot poison the others.
+statistics against a plain torch computation.  Run each stage in its own process so that a trapping kernel
+cannot poison the others.
 
     python tools/gpu_diag.py <stage>      stage in: gemm_small gemm_epi gemm_big attention codec attention_b32
 """
@@ -182,7 +182,7 @@ def main():
         run_gemm(128, 256, 1280, L.EPI_BF16)
         run_gemm(256, 512, 128, L.EPI_BF16)
         run_gemm(300, 512, 256, L.EPI_BF16)
-        run_gemm(40000, 512, 128, L.EPI_BF16)  # > 148 tiles: persistent loop + both accumulators
+        run_gemm(40000, 512, 128, L.EPI_BF16)  # 313 x 2 tiles: more CTAs than SMs
     elif stage == "gemm_epi":
         run_gemm(300, 512, 256, L.EPI_BIAS_F32)
         run_gemm(300, 512, 256, L.EPI_RESID)

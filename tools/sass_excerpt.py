@@ -1,9 +1,9 @@
-"""Per-kernel census of the Blackwell-specific SASS in the built library (run in the authoring container):
+"""Per-kernel census of the Hopper-specific SASS in the built library (no GPU needed):
 
-    python tools/sass_excerpt.py > profiles/sass_r2.txt
+    python tools/sass_excerpt.py > sass.txt
 
-tcgen05.mma -> UTC*MMA, tcgen05.ld/st -> LDTM/STTM, TMA -> UTMALDG/UTMASTG, tcgen05.commit -> UTCBAR, mbarrier -> SYNCS
-(B200_PROFILING.md "What proves a Blackwell-native kernel").  One example line per mnemonic is printed under the counts."""
+wgmma -> HGMMA (its fences and waits -> WARPGROUP.*), TMA -> UTMALDG/UTMASTG (cluster multicast: UTMALDG.*.MULTICAST),
+mbarrier -> SYNCS.  One example line per mnemonic is printed under the counts."""
 import collections
 import os
 import re
@@ -12,8 +12,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "vampnet_b200", "libvampnet_b200.so")
-PAT = re.compile(r"\b(UTC[A-Z0-9]*MMA(?:\.2CTA)?|UTCBAR(?:\.2CTA)?(?:\.MULTICAST)?|UTCCP|LDTM(?:\.x\d+)?|STTM(?:\.x\d+)?|UTMALDG(?:\.\dD)?(?:\.2CTA)?|"
-                 r"UTMASTG(?:\.\dD)?|UBLKCP|UTMAPF|SYNCS\.[A-Z.0-9]+|MUFU\.EX2|FFMA2|FADD2|HMMA)\b")
+PAT = re.compile(r"\b(HGMMA\.\d+x\d+x\d+|WARPGROUP\.[A-Z]+|UTMALDG(?:\.\dD)?(?:\.MULTICAST)?|"
+                 r"UTMASTG(?:\.\dD)?|UBLKCP|UTMAPF|SYNCS\.[A-Z.0-9]+|MUFU\.EX2|HMMA)\b")
 
 
 def main():
@@ -31,10 +31,10 @@ def main():
         m = PAT.search(line)
         if m:
             per[cur][m.group(1)] += 1
-            if "tmem[" in line and "UTC" in m.group(1) and re.search(r"MMA\S*\s+tmem\[", line):
-                per[cur]["(A operand from TMEM)"] += 1
+            if m.group(1).startswith("HGMMA") and re.search(r"HGMMA\S*\s+R\d+, R\d+, gdesc", line):
+                per[cur]["(A operand from registers)"] += 1
             example.setdefault(m.group(1), re.sub(r"/\*[0-9a-f]+\*/", "", line).strip().rstrip(";").strip())
-    print(f"# {os.path.relpath(LIB, ROOT)}: Blackwell-specific SASS per kernel (cuobjdump -sass)")
+    print(f"# {os.path.relpath(LIB, ROOT)}: Hopper-specific SASS per kernel (cuobjdump -sass)")
     for name, c in per.items():
         if not c:
             continue

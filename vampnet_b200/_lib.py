@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/vampnet_b200.h.
 
-The library is built in-tree by ``python -m vampnet_b200.build`` (nvcc, sm_100a).  There is no
+The library is built in-tree by ``python -m vampnet_b200.build`` (nvcc, sm_90a).  There is no
 CPU fallback: if the shared object is missing or cannot be loaded, every entry point raises.
 """
 from __future__ import annotations
@@ -88,14 +88,14 @@ def lib():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        # not a fallback: the only way to get the kernels is to compile them (nvcc cross-compiles sm_100a anywhere)
+        # not a fallback: the only way to get the kernels is to compile them (nvcc cross-compiles sm_90a anywhere)
         try:
             from . import build as _build
             _build.build()
         except Exception as e:
             raise RuntimeError(
                 f"{LIB_PATH} not found and building it failed ({e}); build it with `python -m vampnet_b200.build` "
-                "(nvcc, sm_100a). vampnet_b200 has no CPU or PyTorch fallback.") from e
+                "(nvcc, sm_90a). vampnet_b200 has no CPU or PyTorch fallback.") from e
     L = C.CDLL(LIB_PATH)
     for name, (res, args) in _SIGS.items():
         fn = getattr(L, name)

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library (in-tree, so it travels to the GPU box with the snapshot).
+"""Build the sm_90a (H100) shared library in-tree, next to the package that loads it.
 
     python -m vampnet_b200.build [--force] [--verbose]
 
@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libvampnet_b200.so")
-SOURCES = ["api.cu", "gemm_tcgen05.cu", "attention_tcgen05.cu", "elementwise.cu", "sampler.cu", "codec.cu", "conv_tcgen05.cu"]
+SOURCES = ["api.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "elementwise.cu", "sampler.cu", "codec.cu", "conv_wgmma.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 
@@ -37,7 +37,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     procs = []
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     common = [
-        NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+        NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
         "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
     ]
     if verbose:
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    link = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    link = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -1,4 +1,4 @@
-"""DAC-family neural codec on the sm_100a kernels (SURVEY.md §8a rows D1-D3).
+"""DAC-family neural codec on the sm_90a kernels (SURVEY.md §8a rows D1-D3).
 
 Provides what the reference takes from ``lac.model.lac.LAC`` (imported "as DAC", reference
 vampnet/interface.py:16):  DAC.load, .preprocess, .encode(...)["codes"], .decode(z)["audio"],
@@ -222,7 +222,7 @@ class DAC(nn.Module):
         self.codebook_size = codebook_size
         self.codebook_dim = codebook_dim
         self.sample_rate = sample_rate
-        # "tc": tcgen05 tensor-core convolutions with split-bf16 operands (fp32-grade); "fp32": CUDA-core kernels
+        # "tc": wgmma tensor-core convolutions with split-bf16 operands (fp32-grade); "fp32": CUDA-core kernels
         assert precision in ("tc", "fp32")
         widths = [encoder_dim * 2 ** i for i in range(len(self.encoder_rates) + 1)] + \
                  [decoder_dim // 2 ** i for i in range(len(self.decoder_rates) + 1)]
@@ -301,7 +301,7 @@ class DAC(nn.Module):
         if self._pack is not None:
             return self._pack
         if self.device.type != "cuda":
-            raise RuntimeError("vampnet_b200.codec.DAC runs only on a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("vampnet_b200.codec.DAC runs only on a CUDA (sm_90a) device; there is no CPU fallback")
         P = self.params.get
         L = self.n_codebooks
         q = "quantizer.quantizers."
@@ -442,7 +442,7 @@ class DAC(nn.Module):
     # ---- tensor-core forward passes (activations channels-last, carried as fp32 stream + hi/lo bf16 operand) ----
     def _tc(self, act, base, N, taps, dil, pad, Tq, s=1, alpha=None, alpha_mod=1, resid=None, out_f32=False,
             out_split=True, bias_mod=None, out_rows=None, out_offset=0):
-        """One tcgen05 convolution.  act = (hi, lo) (B, Tin, Cin).  Returns (f32 | None, (hi, lo) | None)."""
+        """One tensor-core convolution.  act = (hi, lo) (B, Tin, Cin).  Returns (f32 | None, (hi, lo) | None)."""
         hi, lo = act
         B, Tin, Cin = hi.shape
         wh, wl = self._pack["tc:" + base]

@@ -365,7 +365,7 @@ int32_t vnb_model_create(const vnb_config* cfg, const vnb_weights* w, vnb_model*
   int dev = 0, major = 0;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return fail("vampnet_b200 needs an sm_100 device (got compute capability major %d)", major);
+  if (major != 9) return fail("vampnet_b200 needs an sm_90 (Hopper) device (got compute capability major %d)", major);
   CK(prepare_gemm());
   auto* m = new vnb_model();
   m->cfg = *cfg;

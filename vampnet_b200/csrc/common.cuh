@@ -1,6 +1,6 @@
-// vampnet_b200 — shared device helpers for the sm_100a kernels (inline PTX, no CUTLASS).
+// vampnet_b200 — shared device helpers for the sm_90a kernels (inline PTX, no CUTLASS).
 //
-// mbarrier / TMA (cp.async.bulk.tensor) / tcgen05 (UMMA, TMEM) wrappers.  Every wait is
+// mbarrier / TMA (cp.async.bulk.tensor) / cluster wrappers; the wgmma wrappers are in wgmma.cuh.  Every wait is
 // bounded: a protocol bug traps (and surfaces as a CUDA error on the host) instead of
 // hanging the device.
 #pragma once
@@ -59,20 +59,17 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: traps with a message when the barrier has not completed after VNB_WAIT_TIMEOUT_NS.
+// Bounded wait: traps when the barrier has not completed after VNB_WAIT_TIMEOUT_NS (a protocol bug surfaces as a CUDA
+// error on the host instead of a hang).  No path contains a function call: a call (printf, a non-inlined slow path)
+// anywhere in a kernel makes ptxas serialise its whole wgmma pipeline.
 #ifndef VNB_WAIT_TIMEOUT_NS
 #define VNB_WAIT_TIMEOUT_NS 4000000000ull
 #endif
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const uint64_t t0 = global_timer_ns();
-  while (!mbar_try_wait(bar, parity)) {
-    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) {
-      printf("[vnb] mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) __trap();
 }
 
 // ---- the same operations on 32-bit shared-window addresses.  A kernel that converts its shared-memory base ONCE
@@ -99,27 +96,17 @@ __device__ __forceinline__ bool mbar_try_wait_a(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// out-of-line slow path: keeps the timeout / printf / trap code out of the callers' instruction streams
-static __device__ __noinline__ void mbar_wait_slow_a(uint32_t bar, uint32_t parity, int tag) {
+__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait_a(bar, parity)) return;
   const uint64_t t0 = global_timer_ns();
-  while (!mbar_try_wait_a(bar, parity)) {
-    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) {
-      printf("[vnb] mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity, int tag = 0) {
-  if (!mbar_try_wait_a(bar, parity)) mbar_wait_slow_a(bar, parity, tag);
+  while (!mbar_try_wait_a(bar, parity))
+    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) __trap();
 }
 
 // ------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -159,72 +146,10 @@ __device__ __forceinline__ void bulk_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------ TMEM alloc
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(kCols) : "memory");
-}
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor, K-major operand stored as rows of 128 bytes (64 bf16)
-// with the 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 B
-// apart (SBO), LBO is unused for swizzled K-major layouts, version field = 1 (sm_100).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);       // start address, bits [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                          // LBO (ignored), bits [16,30)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // SBO = 1024 B, bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                          // descriptor version 1
-  d |= static_cast<uint64_t>(2) << 61;                          // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16, A/B = bf16 (K-major both), D = fp32.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same with the A operand read from TENSOR MEMORY (128 lanes = rows, K-major: 32-bit column c holds elements 2c, 2c+1 as
-// a bf16 pair, low half first), B from shared memory.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// ------------------------------------------------------------------ CTA pair (cta_group::2) variants
-// Two CTAs of a cluster on one TPC issue ONE tcgen05.mma of M=256: each holds 128 rows of A and N/2 rows of B in
-// its own shared memory and receives its 128 accumulator rows in its own TMEM.  Only the rank-0 CTA issues the
-// MMA; its mbarriers collect the TMA bytes of both CTAs, commits are multicast to both.
+// ------------------------------------------------------------------ clusters
+// The paired GEMM runs as clusters of two CTAs that share one W tile: each CTA fetches half of it and the TMA
+// multicasts that half into both CTAs' shared memory; a stage is refilled only when the consumers of both CTAs
+// have released it (remote mbarrier arrivals).
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -242,12 +167,6 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t cta_addr, uint32_t rank) {
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-// Same arrival with the default (.release, .cta-scope) semantics: no MEMBAR.ALL.GPU in front of it.  Enough when the
-// only thing the waiter depends on is work that has already COMPLETED in the arriving thread (tcgen05.ld followed by
-// tcgen05.wait::ld), not memory the waiter is going to read.
-__device__ __forceinline__ void mbar_arrive_remote_cta(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
 __device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -259,91 +178,22 @@ __device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t pa
       : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity, int tag = 0) {
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait_cluster(bar, parity)) return;
   const uint64_t t0 = global_timer_ns();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) {
-      printf("[vnb] cluster mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x,
-             blockIdx.y, blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait_cluster(bar, parity))
+    if (global_timer_ns() - t0 > VNB_WAIT_TIMEOUT_NS) __trap();
 }
-// TMA into THIS CTA's shared memory, bytes credited to an mbarrier given by its shared::cluster address
-// (the rank-0 CTA's barrier).
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
+// TMA multicast: the box lands at the same shared-memory offset `dst` in every CTA of `cta_mask`, and each of them has
+// its bytes credited to its own mbarrier at offset `bar`.
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                               uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem) {  // the same warp of BOTH CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t addr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the mbarrier at this offset in BOTH CTAs when the MMAs issued so far have completed.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-
-// ------------------------------------------------------------------ TMEM <-> registers
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ small math / packing
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -374,25 +224,6 @@ __device__ __forceinline__ void sts_f4(uint32_t addr, float4 v) {
 }
 __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-// packed fp32x2 arithmetic (Blackwell FFMA2 / FADD2): two lanes per issue slot
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
 }
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll

@@ -7,7 +7,7 @@ namespace vnb {
 
 // ------------------------------------------------------------------------------------------------
 // CodebookEmbedding.from_codes (reference vampnet/modules/layers.py:134-156) as the A operand of the out_proj
-// contraction (:162), which runs on the tensor cores (gemm_tcgen05_kernel<BIAS_F32>, api.cu):
+// contraction (:162), which runs on the tensor cores (gemm_wgmma_kernel<BIAS_F32>, api.cu):
 //   latent[m, c*8 + j] = table[c][code[m, c]][j]        (code == V selects the learned MASK row)
 //   A[m, :] = [ hi(latent) | hi(latent) | lo(latent) ]   bf16, each third zero-padded to Kp columns
 // so that A . [w_hi | w_lo | w_hi]^T = latent . w to fp32 accuracy (split-bf16: hi = bf16(v), lo = bf16(v - hi)).
@@ -48,7 +48,8 @@ cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, 
   if (K > Kp || ss_parts - zero_from > Kp) return cudaErrorInvalidValue;
   const long long total = static_cast<long long>(M) * Kp;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  const long long cap = 16LL * device_sm_count();
+  if (blocks > cap) blocks = cap;
   if (codes_btc != nullptr)
     embed_gather_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, st>>>(codes_btc, nullptr, table,
                                                                              reinterpret_cast<__nv_bfloat16*>(A), M, T, C, V1, K,

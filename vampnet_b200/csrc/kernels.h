@@ -49,13 +49,13 @@ struct SampleDyn;
 // ---- GEMM ----
 struct GemmPlan {
   CUtensorMap tmA, tmB;
-  CUtensorMap tmBh;  // W with a 128-row box: the half tile each CTA of a pair stages (gemm_tcgen05.cu, PAIR)
+  CUtensorMap tmBh;  // W with a 128-row box: the half tile each CTA of a pair fetches and multicasts (gemm_wgmma.cu, PAIR)
   int M = 0, N = 0, K = 0, epi = 0;
   void* out = nullptr;
   void* out2 = nullptr;
   const float* bias = nullptr;
   int T = 1, Tpad = 1, d2 = 0;
-  // fused RMSNorm plumbing (see GemmArgs in gemm_tcgen05.cu)
+  // fused RMSNorm plumbing (see GemmArgs in gemm_wgmma.cu)
   void* out_bf16 = nullptr;
   float* ss_out = nullptr;
   const float* ss_in = nullptr;
@@ -73,7 +73,7 @@ bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, i
 bool gemm_plan_set_fused_out(GemmPlan* p, void* out_bf16, float* ss_out);
 cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st);
 cudaError_t prepare_gemm();  // per-device kernel attributes; call outside stream capture
-void set_gemm_pair(int on);  // 1: CTA-pair (cta_group::2) GEMM tiles, 0: single-CTA tiles
+void set_gemm_pair(int on);  // 1: CTA pairs (clusters of two sharing the W tile), 0: single-CTA tiles
 int get_gemm_pair();
 int get_gemm_max_clusters();  // co-resident CTA pairs of the pair kernel on the current device
 cudaError_t launch_gemm_ref(const void* A, const void* W, int M, int N, int K, float* out, cudaStream_t st);

@@ -3,7 +3,7 @@
 // result is discarded by the reference and so is absent here), the where()s that keep known tokens,
 // the cosine-schedule count (:903-913, mask.py:8-9) and mask_by_random_topk (:1038-1074).
 //
-// In the generate loop the draw itself happens inside the classifier GEMM's epilogue (gemm_tcgen05.cu, EPI_SAMPLE: the
+// In the generate loop the draw itself happens inside the classifier GEMM's epilogue (gemm_wgmma.cu, EPI_SAMPLE: the
 // logits never reach HBM); what runs here afterwards:
 //   sample_combine_kernel  one thread per (batch, position): picks the 128-entry vocabulary tile from the per-tile
 //                          records the epilogue left (uniform 1), takes that tile's candidate, writes token + confidence.
@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
                   dyn.seed_hi, r);
     // Two-level inverse CDF (oracle/vampnet_oracle.py sample_from_logits, rng="philox"): uniform 1 picks the
     // 128-entry tile (= chunk i of this layout) by its mass, uniform 2 the entry inside it.  The classifier GEMM's
-    // sampling epilogue (gemm_tcgen05.cu, EPI_SAMPLE) draws the same way from its own 128-column strips.
+    // sampling epilogue (gemm_wgmma.cu, EPI_SAMPLE) draws the same way from its own 128-column strips.
     const float target = u01(r[0]) * se;  // tile = first i with cumsum(tile mass)[i] > target
     const float u2 = u01(r[1]);
     float base = 0.f;
@@ -322,7 +322,7 @@ __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, cons
   }
 }
 
-// Second half of the fused path.  The classifier GEMM's sampling epilogue (gemm_tcgen05.cu, EPI_SAMPLE) left one
+// Second half of the fused path.  The classifier GEMM's sampling epilogue (gemm_wgmma.cu, EPI_SAMPLE) left one
 // 16-byte record per (row, 128-entry vocabulary tile): {tile max of the logits, sum of exp((x - max) / temperature),
 // logit of the tile's candidate, candidate | arg-max << 16 (vocabulary indices)}; the candidate was drawn inside the tile
 // with uniform 2.  One thread per row: pick the tile with uniform 1 by mass, take its candidate, and compute

@@ -1,7 +1,7 @@
 """Interface — drop-in for the reference's ``vampnet.interface.Interface`` surface
 (reference vampnet/interface.py:54-562): checkpoint loading, encode, build_mask, chunked coarse_vamp,
 coarse_to_fine, vamp, decode.  Same method names, arguments, defaults, return types and error behaviour;
-the compute underneath is the sm_100a CUDA path (VampNet.generate, the codec kernels).
+the compute underneath is the sm_90a CUDA path (VampNet.generate, the codec kernels).
 
 Chunk loops are kept (they define the reference's results: every chunk is an independent generate() call
 with its own whole-batch N0), but each chunk's loop body is one CUDA-graph replay.

@@ -1,5 +1,5 @@
 """VampNet — drop-in for the reference's ``vampnet.modules.transformer.VampNet`` surface
-(reference vampnet/modules/transformer.py:535-946) whose compute runs in hand-written sm_100a
+(reference vampnet/modules/transformer.py:535-946) whose compute runs in hand-written sm_90a
 CUDA behind the C ABI (include/vampnet_b200.h).
 
 The nn.Module tree below only *holds parameters* under the reference's state_dict key names
@@ -201,7 +201,7 @@ class VampNet(nn.Module):
         self.embedding_dim = embedding_dim
         self.vocab_size = vocab_size
         self.latent_dim = latent_dim
-        self.flash_attn = flash_attn  # accepted and ignored: attention is always the fused sm_100a kernel
+        self.flash_attn = flash_attn  # accepted and ignored: attention is always the fused sm_90a kernel
         self.noise_mode = noise_mode
         self.cond_dim = cond_dim
         self.dropout = dropout
@@ -378,7 +378,7 @@ class VampNet(nn.Module):
 
     def _ensure_handle(self, codec):
         if self.device.type != "cuda":
-            raise RuntimeError("vampnet_b200.VampNet runs only on a CUDA (sm_100a) device; there is no CPU fallback. "
+            raise RuntimeError("vampnet_b200.VampNet runs only on a CUDA (sm_90a) device; there is no CPU fallback. "
                                "Move the model with .to('cuda').")
         key = (id(codec), str(self.device))
         if self._handle is not None and self._packed_key == key:
