@@ -9,7 +9,9 @@
 // One CTA = (batch, head, 128 queries), 64-key blocks, two CTAs per SM:
 //   warp 8      TMA producer: Q once; K_j and V^T_j through a 3-stage ring
 //   warps 0..7  two consumer warpgroups, 64 query rows each.  Per key block: S = Q.K_j^T (wgmma, both operands in shared
-//               memory, 32 fp32 scores per thread) -> online softmax in registers (exp2 domain; a row's four threads
+//               memory, 32 fp32 scores per thread) -> bias: one table value for a block wholly beyond +-sat from
+//               the warp's rows, else an unclamped lookup in an edge-padded table; the key < T mask only in a ragged
+//               last block -> online softmax in registers (exp2 domain; a row's four threads
 //               exchange maxima and sums by shuffles) -> P packed to bf16 in registers, which is exactly the A-operand
 //               fragment of the next wgmma -> O += P.V_j (wgmma with A from registers, B = V^T_j in shared memory).
 //               O (64 x 64 fp32) stays in registers for the whole key loop.
@@ -27,7 +29,8 @@ constexpr int Q_BYTES = AQ * DH * 2;        // 16 KiB
 constexpr int K_BYTES = AK * DH * 2;        // 8 KiB
 constexpr int V_BYTES = DH * AK * 2;        // 8 KiB
 constexpr int MAX_SAT = 128;
-constexpr int TAB = 2 * MAX_SAT + 1;
+constexpr int PAD = 80;                     // edge copies on each side of the table: >= one key block + a warp's rows
+constexpr int TAB = 2 * MAX_SAT + 1 + 2 * PAD;
 constexpr int THREADS = 256 + 32;
 constexpr float LOG2E = 1.4426950408889634f;
 
@@ -73,8 +76,11 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     }
     mbar_fence_init();
   }
-  // bias table of this head, times log2(e): entry [rel + sat] for rel in [-sat, sat]
-  for (int i = threadIdx.x; i <= 2 * sat; i += THREADS) sts_f32(sb + OFF_BIAS + 4u * i, a.rel[i * a.H + h] * LOG2E);
+  // bias table of this head, times log2(e): entry [rel + sat + PAD] for rel in [-sat - PAD, sat + PAD], clamped
+  for (int i = threadIdx.x; i <= 2 * (sat + PAD); i += THREADS) {
+    const int e = min(max(i - PAD, 0), 2 * sat);
+    sts_f32(sb + OFF_BIAS + 4u * i, a.rel[e * a.H + h] * LOG2E);
+  }
   __syncthreads();
 
   if (warp == 8) {
@@ -98,10 +104,12 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   // Accumulator fragment of m64nNk16: thread (warp w of the warpgroup, lane l) holds rows 16 w + l/4 (regs 4i, 4i+1)
   // and 16 w + l/4 + 8 (regs 4i+2, 4i+3), columns 8 i + 2 (l % 4) + {0, 1}.
   const int wg = warp >> 2;
-  const int qr = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // query of this thread's first row (second: qr + 8)
+  const int qw = q0 + wg * 64 + (warp & 3) * 16;                // first query row of this warp
+  const int qr = qw + (lane >> 2);                               // query of this thread's first row (second: qr + 8)
   const int kc = 2 * (lane & 3);                                 // first key column of this thread inside an n8 block
   const uint32_t sQ = sb + OFF_Q + wg * (64 * 128);
   const float c = 0.125f * LOG2E;                                // 1/sqrt(64) folded with log2(e)
+  const bool ragged = (a.T % AK) != 0;
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -121,23 +129,45 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     wgmma_wait<0>();
     wgmma_fence_regs(s);
 
-    // t = score * c + bias[k - q] (log2 domain); keys beyond T -> -inf
+    // t = score * c + bias[clamp(k - q)] (log2 domain); keys beyond T -> -inf.  A warp's 16 rows against a 64-key
+    // block span k - q in [lo, lo + 78]: wholly at or beyond -sat or +sat the bias is one table entry; otherwise the
+    // index k - q + sat + PAD stays inside the edge-padded table and needs no clamp.
+    const int lo = j * AK - qw - 15;
+    if (ragged && j == nblk - 1) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = j * AK + 8 * i + kc + e;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            int rel = key - (qr + 8 * r);
+            rel = rel < -sat ? -sat : (rel > sat ? sat : rel);
+            float t = __fmaf_rn(s[4 * i + 2 * r + e], c, lds_f32(sb + OFF_BIAS + 4u * (rel + sat + PAD)));
+            if (key >= a.T) t = -INFINITY;
+            s[4 * i + 2 * r + e] = t;
+          }
+        }
+      }
+    } else if (lo + 78 <= -sat || lo >= sat) {
+      const float bc = lds_f32(sb + OFF_BIAS + 4u * (lo >= sat ? 2 * sat + PAD : PAD));  // bias[+-sat]
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = __fmaf_rn(s[i], c, bc);
+    } else {
+      const uint32_t tb = sb + OFF_BIAS + 4u * (j * AK + kc - qr + sat + PAD);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int r = 0; r < 2; ++r)
+            s[4 * i + 2 * r + e] = __fmaf_rn(s[4 * i + 2 * r + e], c, lds_f32(tb + 4 * (8 * i + e - 8 * r)));
+    }
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int key = j * AK + 8 * i + kc + e;
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          int rel = key - (qr + 8 * r);
-          rel = rel < -sat ? -sat : (rel > sat ? sat : rel);
-          float t = __fmaf_rn(s[4 * i + 2 * r + e], c, lds_f32(sb + OFF_BIAS + 4u * (rel + sat)));
-          if (key >= a.T) t = -INFINITY;
-          s[4 * i + 2 * r + e] = t;
-          mx[r] = fmaxf(mx[r], t);
-        }
-      }
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
     }
     float alpha[2];
 #pragma unroll
@@ -149,16 +179,20 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       m[r] = m_new;
       l[r] *= alpha[r];
     }
-    // P = exp2(t - m) packed as bf16 pairs: key chunk kk (16 keys) = n8 blocks 2kk, 2kk+1 = the A fragment of k-step kk
+    // P = exp2(t - m), in place
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      s[4 * i] = fast_exp2(s[4 * i] - m[0]); s[4 * i + 1] = fast_exp2(s[4 * i + 1] - m[0]);
+      s[4 * i + 2] = fast_exp2(s[4 * i + 2] - m[1]); s[4 * i + 3] = fast_exp2(s[4 * i + 3] - m[1]);
+      l[0] += s[4 * i] + s[4 * i + 1];
+      l[1] += s[4 * i + 2] + s[4 * i + 3];
+    }
+    // P packed as bf16 pairs: key chunk kk (16 keys) = n8 blocks 2kk, 2kk+1 = the A fragment of k-step kk
     uint32_t p[4][4];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const float p00 = fast_exp2(s[4 * i] - m[0]), p01 = fast_exp2(s[4 * i + 1] - m[0]);
-      const float p10 = fast_exp2(s[4 * i + 2] - m[1]), p11 = fast_exp2(s[4 * i + 3] - m[1]);
-      l[0] += p00 + p01;
-      l[1] += p10 + p11;
-      p[i >> 1][(i & 1) * 2] = pack_bf16x2(p00, p01);
-      p[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(p10, p11);
+      p[i >> 1][(i & 1) * 2] = pack_bf16x2(s[4 * i], s[4 * i + 1]);
+      p[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(s[4 * i + 2], s[4 * i + 3]);
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
