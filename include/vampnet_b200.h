@@ -161,6 +161,31 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
                          int32_t B, int32_t T, int32_t Tpad, int32_t H, void* stream);
 /* Naive SIMT GEMM used only to bisect the tensor-core path in tests: out fp32 (M, N) = A x W^T. */
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream);
+/* Test-only: vnb_op_gemm plus the fused-RMSNorm plumbing the forward uses, epi in {BF16, QKV, RESID, GEGLU, BIAS_F32}.
+ * Consumer side: ss_in (ss_parts, M) fp32 or NULL; every accumulator row m is scaled by
+ *   rs = rsqrt(sum_{p < ss_parts} ss_in[p*M + m] * inv_d + eps)   (partials added in order p = 0, 1, ...)
+ * before the epilogue's own operation (GEGLU: value and gate; QKV: qk and vT; BIAS_F32: before the bias).
+ * Producer side (RESID and BIAS_F32 only, both or neither, error otherwise): out_bf16 (M, N) bf16 = bf16(out) and
+ * ss_out fp32 row sums of squares of out, part p at ss_out[p*M + m]:
+ *   RESID     2 parts per 256-column tile j: part 2j over its 32-column chunks {0, 2, 4, 6}, part 2j+1 over {1, 3, 5, 7}
+ *             (N/128 parts in all);
+ *   BIAS_F32  1 part per 256-column tile (N/256 parts); nothing else is written. */
+int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                           void* out2, const float* bias, int32_t T, int32_t Tpad, const float* ss_in,
+                           int32_t ss_parts, float inv_d, float eps, void* out_bf16, float* ss_out, void* stream);
+/* Test-only: the classifier GEMM with the sampling epilogue of the generate loop (VNB_EPI_SAMPLE) alone.
+ * N == (C - ncc) * V, V % 128 == 0, V <= 1024; logits x = (A . W^T) * rs + bias with rs as above.
+ * zcur (M, C) int32, row m = b*T + t: codebook ncc + cp of row m is sampled iff it holds mask_token.
+ * partials (M * (C-ncc) * V/128) float4: for every sampled (row m, codebook cp, 128-entry tile k), record
+ * (m*(C-ncc) + cp) * V/128 + k = {max x, sum exp((x - max) / temperature), x of the candidate, candidate | argmax << 16}
+ * (vocabulary indices; argmax: lowest index on ties; candidate: first entry whose running sum exceeds u * sum, u the
+ * second Philox uniform of counter (t*(C-ncc) + cp, b, step, 0) and key (seed_lo, seed_hi), the argmax when do_sample
+ * is 0).  Records of known positions are not written.  temperature <= 0 means 1. */
+int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,
+                            const float* ss_in, int32_t ss_parts, float inv_d, float eps, const int32_t* zcur,
+                            int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token, float temperature,
+                            int32_t do_sample, int32_t step, uint32_t seed_lo, uint32_t seed_hi, void* partials,
+                            void* stream);
 
 /* ---- codec (DAC family; reference call sites: interface.py:223 codec.encode, transformer.py:671-675
  *      codec.quantizer.from_latents + codec.decode).  fp32, (B, C, T) channels-first. ------------------------

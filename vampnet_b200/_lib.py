@@ -73,6 +73,13 @@ _SIGS = {
     "vnb_codec_conv_out": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32] * 5 + [C.c_void_p]),
     "vnb_set_error_cuda": (C.c_int32, [C.c_char_p, C.c_int32]),
     "vnb_dbg_gemm_ref": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_dbg_gemm_fused": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float,
+                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_dbg_gemm_sample": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,
+                                        C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

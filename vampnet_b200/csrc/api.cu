@@ -342,6 +342,28 @@ static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st
   return 0;
 }
 
+// temperature <= 0: softmax(logits) without scaling (transformer.py:1019-1023)
+static float inv_temperature(float temperature) {
+  return temperature > 0.f ? static_cast<float>(1.0 / static_cast<double>(temperature)) : 1.0f;
+}
+
+// The single-step entry points take their SampleDyn from a per-device ring of 64 device slots (a process-global ring
+// would live on whichever device called first); each call stages its scalars into the next slot, stream-ordered.
+static int stage_sample_dyn(const SampleDyn& d, cudaStream_t st, const SampleDyn** out) {
+  static SampleDyn* scratch_dev[64] = {nullptr};
+  static int slot_dev[64] = {0};
+  int dev = 0;
+  CK(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return fail("device index %d out of range", dev);
+  SampleDyn*& scratch = scratch_dev[dev];
+  int& slot = slot_dev[dev];
+  if (!scratch) CK(cudaMalloc(&scratch, sizeof(SampleDyn) * 64));
+  SampleDyn* dd = scratch + (slot++ & 63);
+  CK(cudaMemcpyAsync(dd, &d, sizeof(d), cudaMemcpyHostToDevice, st));
+  *out = dd;
+  return 0;
+}
+
 }  // namespace vnb
 
 using namespace vnb;
@@ -465,7 +487,7 @@ int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_
   m->last = ws;
   const int steps = p->sampling_steps;
   std::vector<SampleDyn> dyn(steps);
-  const float inv_t = p->temperature > 0.f ? static_cast<float>(1.0 / static_cast<double>(p->temperature)) : 1.0f;
+  const float inv_t = inv_temperature(p->temperature);
   for (int i = 0; i < steps; ++i) {
     dyn[i].inv_temp = inv_t;
     dyn[i].gamma = p->gamma[i];
@@ -584,21 +606,12 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
                         int32_t do_sample, float temperature, float gamma, float temp_eff, uint32_t seed_lo,
                         uint32_t seed_hi, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // per-device ring of parameter slots (a process-global one would live on whichever device called first)
-  static SampleDyn* scratch_dev[64] = {nullptr};
-  static int slot_dev[64] = {0};
-  int dev = 0;
-  CK(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return fail("device index %d out of range", dev);
-  SampleDyn*& scratch = scratch_dev[dev];
-  int& slot = slot_dev[dev];
-  if (!scratch) CK(cudaMalloc(&scratch, sizeof(SampleDyn) * 64));
   SampleDyn d;
-  d.inv_temp = temperature > 0.f ? static_cast<float>(1.0 / static_cast<double>(temperature)) : 1.0f;
+  d.inv_temp = inv_temperature(temperature);
   d.gamma = gamma; d.temp_eff = temp_eff; d.do_sample = do_sample; d.is_last = is_last; d.step = step;
   d.seed_lo = seed_lo; d.seed_hi = seed_hi; d.top_p = 0.f;
-  SampleDyn* dd = scratch + (slot++ & 63);
-  CK(cudaMemcpyAsync(dd, &d, sizeof(d), cudaMemcpyHostToDevice, st));
+  const SampleDyn* dd = nullptr;
+  if (stage_sample_dyn(d, st, &dd)) return 1;
   SampleArgs sa;
   sa.logits = logits; sa.zcur = zflat; sa.zorig = nullptr; sa.tokens = tokens_out; sa.conf = conf_out; sa.n0 = n0;
   sa.B = B; sa.T = S; sa.C = 1; sa.ncc = 0; sa.V = V; sa.mask_token = mask_token;
@@ -624,6 +637,49 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
 }
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream) {
   CK(launch_gemm_ref(A, W, M, N, K, out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+// The plans below are built exactly as get_workspace() builds the forward's (make_gemm_plan, then the consumer fields
+// or gemm_plan_set_fused_out), so the tests reach every epilogue branch the forward launches.
+int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                           void* out2, const float* bias, int32_t T, int32_t Tpad, const float* ss_in,
+                           int32_t ss_parts, float inv_d, float eps, void* out_bf16, float* ss_out, void* stream) {
+  if (epi < VNB_EPI_BF16 || epi > VNB_EPI_BIAS_F32) return fail("vnb_dbg_gemm_fused: epilogue %d not supported", epi);
+  if ((out_bf16 != nullptr || ss_out != nullptr) && epi != VNB_EPI_RESID && epi != VNB_EPI_BIAS_F32)
+    return fail("vnb_dbg_gemm_fused: out_bf16 / ss_out need the RESID or BIAS_F32 epilogue");
+  if ((out_bf16 == nullptr) != (ss_out == nullptr)) return fail("vnb_dbg_gemm_fused: out_bf16 and ss_out go together");
+  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_fused: ss_parts must be >= 1");
+  if (epi == VNB_EPI_BIAS_F32 && bias == nullptr) return fail("vnb_dbg_gemm_fused: BIAS_F32 needs a bias");
+  if (epi == VNB_EPI_QKV && (out2 == nullptr || N % 96 != 0 || T < 1 || Tpad < T))
+    return fail("vnb_dbg_gemm_fused: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
+  GemmPlan p;
+  const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
+  if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
+  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
+  if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
+  CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,
+                            const float* ss_in, int32_t ss_parts, float inv_d, float eps, const int32_t* zcur,
+                            int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token, float temperature,
+                            int32_t do_sample, int32_t step, uint32_t seed_lo, uint32_t seed_hi, void* partials,
+                            void* stream) {
+  if (V % 128 != 0 || V > 1024 || ncc < 0 || C <= ncc || N != (C - ncc) * V || T < 1)
+    return fail("vnb_dbg_gemm_sample: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1");
+  if (!bias || !zcur || !partials) return fail("vnb_dbg_gemm_sample: bias, zcur and partials are required");
+  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_sample: ss_parts must be >= 1");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  SampleDyn d = {};
+  d.inv_temp = inv_temperature(temperature);
+  d.do_sample = do_sample; d.step = step; d.seed_lo = seed_lo; d.seed_hi = seed_hi;
+  GemmPlan p;
+  if (!make_gemm_plan(&p, VNB_EPI_SAMPLE, A, W, M, N, K, nullptr, nullptr, bias, T, T, 0))
+    return fail("gemm plan: %s", tmap_error());
+  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
+  p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
+  if (stage_sample_dyn(d, st, &p.dyn)) return 1;
+  CK(launch_gemm(p, st));
   return 0;
 }
 

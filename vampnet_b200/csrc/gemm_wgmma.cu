@@ -54,8 +54,10 @@ struct GemmArgs {
   int T, Tpad;        // EPI_QKV: rows m = b*T + t
   int d2;             // EPI_QKV: 2*d_model (column where V starts)
   // ---- fused RMSNorm (reference transformer.py:43-58), see DESIGN.md §4 ----
-  __nv_bfloat16* out_bf16;  // EPI_RESID: bf16 copy of the updated residual stream (A operand of the next GEMM)
-  float* ss_out;            // EPI_RESID: (N/256, M) per-n-tile partial row sums of squares of the updated rows
+  __nv_bfloat16* out_bf16;  // EPI_RESID / EPI_BIAS_F32: bf16 copy of the fp32 output (A operand of the next GEMM)
+  float* ss_out;            // partial row sums of squares of the fp32 output, part p at [p * M + row]: EPI_RESID
+                            // (N/128, M), parts 2j / 2j+1 = even / odd 32-column chunks of n-tile j; EPI_BIAS_F32
+                            // (N/256, M), one part per n-tile
   const float* ss_in;       // consumers: partial row sums of squares of THEIR A operand; null = no row scaling
   int ss_parts;             // number of partials to add (fixed order: deterministic)
   float inv_d, eps;         // row scale = rsqrt(sum * inv_d + eps)
