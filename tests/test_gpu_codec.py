@@ -98,3 +98,98 @@ def test_cpu_codec_raises():
     m = DAC(encoder_dim=32, decoder_dim=512)
     with pytest.raises(RuntimeError, match="no CPU fallback"):
         m.encode(torch.zeros(1, 1, 768))
+
+
+def test_odd_decoder_rate_matches_oracle_length():
+    """ConvTranspose1d(2s, stride s, pad ceil(s/2)) gives T*s - s % 2 samples: with rates (3, 2), 5 frames decode to
+    29 samples.  Both precisions must return the oracle's length and values."""
+    cfg = do.CodecConfig(encoder_dim=32, decoder_dim=256, encoder_rates=(3, 2))
+    zq = torch.randn(2, cfg.latent_dim, 5, generator=torch.Generator().manual_seed(6))
+    w = do.make_codec_weights(cfg, seed=0)
+    ref = do.decode(zq, w, cfg)["audio"]
+    assert ref.shape == (2, 1, 29)
+    for precision in PRECISIONS:
+        _, m = build(cfg, precision=precision)
+        got = m.decode(zq.cuda())["audio"].cpu()
+        assert got.shape == ref.shape, (precision, got.shape)
+        err = (got - ref).abs().max().item()
+        print(f"odd rates, {precision}: max err {err:.3e}")
+        assert err < 2e-4
+
+
+# ---- config [3]'s clip length: 32 ten-second clips of 441 000 samples (441 600 after padding, 575 frames)
+TEN_S = 441_000
+EN_ERR_MAX = 5e-4   # L2 error of the normalised latents; measured 2.0e-4 on an H100, so delta <= 2e-3
+
+
+@pytest.fixture(scope="module")
+def ten_second():
+    from tools.codec_bits import full_codec
+    cfg, w, m = full_codec(seed=0)
+    x = torch.randn(2, 1, TEN_S, generator=torch.Generator().manual_seed(7)) * 0.3
+    xp, n = do.preprocess(x, cfg)
+    assert xp.shape[-1] == 441_600 and xp.shape[-1] // cfg.hop_length == 575
+    return cfg, w, m, xp
+
+
+def test_ten_second_clip_against_float64(ten_second):
+    """Encode (B = 2) and decode at the benchmarked clip length against the oracle run in float64 on the GPU, one row
+    at a time to bound memory: each row's reference zq is decoded at B = 1 by both sides (B = 2 decode equals the rows
+    bit for bit, see the next test).  Codes must agree up to near-ties (tests/codec_op_ref.code_divergence) whose bound
+    delta follows from the kernel's normalised-latent error; that error is itself capped at EN_ERR_MAX, so a codec
+    that loses accuracy cannot widen delta to hide real code errors.  Latents on every comparable level must stay within
+    1e-3, and the decoded waveform within 1e-3 of the float64 decode (DESIGN.md section 2)."""
+    import time
+    from tests import codec_op_ref as R
+    cfg, w, m, xp = ten_second
+    w64 = {k: v.double().cuda() for k, v in w.items()}
+    L = cfg.n_codebooks
+    q = "quantizer.quantizers."
+    win = torch.stack([w64[f"{q}{i}.in_proj.weight"][:, :, 0] for i in range(L)])
+    bin_ = torch.stack([w64[f"{q}{i}.in_proj.bias"] for i in range(L)])
+    wout = torch.stack([w64[f"{q}{i}.out_proj.weight"][:, :, 0] for i in range(L)])
+    bout = torch.stack([w64[f"{q}{i}.out_proj.bias"] for i in range(L)])
+    cb = torch.stack([w64[f"{q}{i}.codebook.weight"] for i in range(L)])
+    enc = m.encode(xp.cuda())
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.time()
+    audio_err, lat_err, en_err, n_div = [], 0.0, 0.0, 0
+    for b in range(xp.shape[0]):
+        with torch.no_grad():
+            z64 = do.encoder(xp[b:b + 1].double().cuda(), w64, cfg)
+            ref = R.rvq(0, z64, None, win, bin_, wout, bout, cb, torch.nn.functional.normalize(cb, dim=-1), L)
+            dv = R.code_divergence(enc["codes"][b:b + 1], enc["latents"][b:b + 1], ref)
+            print(f"row {b}: {int((dv['first'] < L).sum())} of 575 frames diverge (first at level "
+                  f"{int(dv['first'].min())}), normalised-latent err {dv['err_en']:.3e}, delta {dv['delta']:.3e}, "
+                  f"max gap {dv['gap'].max().item():.3e}")
+            assert dv["err_en"] <= EN_ERR_MAX, "normalised latents too far from float64 for the near-tie rule"
+            assert (dv["gap"] < dv["delta"]).all(), "a code differs from float64 by more than a near-tie"
+            n_div += int((dv["first"] < L).sum())
+            en_err = max(en_err, dv["err_en"])
+            d = (enc["latents"][b:b + 1].double() - ref["latents"]).abs().view(1, L, 8, -1).amax(2)   # (1, L, T)
+            lat_err = max(lat_err, d[dv["comparable"]].max().item())
+            audio64 = do.decoder(ref["zq"], w64, cfg)
+            audio = m.decode(ref["zq"].float())["audio"]
+            assert audio.shape == audio64.shape == (1, 1, 441_600)
+            audio_err.append((audio.double() - audio64).abs())
+            del z64, ref, audio64
+    err = torch.cat(audio_err, 0)
+    print(f"ten-second clip: latents max err {lat_err:.3e} (comparable levels), normalised-latent err "
+          f"{en_err:.3e}; waveform max err {err.max().item():.3e}, "
+          f"mean {err.mean().item():.3e}; {n_div} diverging frames; float64 reference {time.time() - t0:.1f} s, "
+          f"peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB")
+    assert lat_err < 1e-3
+    assert err.max().item() <= 1e-3
+
+
+def test_ten_second_clip_batch_rows_match_single_clips(ten_second):
+    """Each row of a B = 2 encode (codes, z) and decode (audio) equals its own B = 1 run, bit for bit."""
+    cfg, w, m, xp = ten_second
+    enc = m.encode(xp.cuda())
+    audio = m.decode(enc["z"])["audio"]
+    for b in range(2):
+        one = m.encode(xp[b:b + 1].cuda())
+        assert torch.equal(one["codes"], enc["codes"][b:b + 1])
+        assert torch.equal(one["z"].view(torch.int32), enc["z"][b:b + 1].contiguous().view(torch.int32))
+        a1 = m.decode(enc["z"][b:b + 1])["audio"]
+        assert torch.equal(a1.view(torch.int32), audio[b:b + 1].view(torch.int32))

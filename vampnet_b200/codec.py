@@ -504,7 +504,7 @@ class DAC(nn.Module):
         return {"z": zq_cl.permute(0, 2, 1), "codes": codes, "latents": lat, "length": N}
 
     def _decode_tc(self, z):
-        """z: (B, latent, T) fp32 (the reference's layout) -> audio (B, 1, T*hop)."""
+        """z: (B, latent, T) fp32 (the reference's layout) -> audio (B, 1, T*hop), or shorter for odd decoder rates."""
         P = self.params.get
         lib = _lib.lib()
         with torch.cuda.device(self.device):
@@ -518,10 +518,12 @@ class DAC(nn.Module):
                 p = f"decoder.block.{i}"
                 co = c // 2
                 pad = math.ceil(s / 2)
-                # transposed conv as ONE GEMM with N = s*Cout phase-major columns and taps (x[q], x[q-1])
+                # transposed conv as ONE GEMM with N = s*Cout phase-major columns and taps (x[q], x[q-1]); its output has
+                # (T-1)*s - 2*pad + 2*s = T*s - s % 2 rows (ConvTranspose1d), so odd strides drop the last row
+                rows = T * s - s % 2
                 skip, act = self._tc(act, p + ".conv_t1", s * co, 2, -1, 0, T + 1, alpha=P(p + ".res_unit1.snake1.alpha"),
-                                     alpha_mod=co, out_f32=True, bias_mod=co, out_rows=T * s, out_offset=-pad * co)
-                T *= s
+                                     alpha_mod=co, out_f32=True, bias_mod=co, out_rows=rows, out_offset=-pad * co)
+                T = rows
                 for r, dil in enumerate((1, 3, 9)):
                     if r < 2:
                         nxt = P(f"{p}.res_unit{r + 2}.snake1.alpha")
