@@ -102,6 +102,28 @@ int32_t vnb_get_hidden(vnb_model* m, float* out, void* stream);
  * out: (B, C, T) int64. */
 int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
                      const vnb_gen_params* p, int64_t* out, void* stream);
+/* One generate() call of a vnb_generate_many launch: `rows` consecutive batch rows with their own sampling state.
+ * The fields mean what the vnb_gen_params fields of the same names mean. */
+typedef struct vnb_gen_group {
+  int32_t rows;
+  float temperature;
+  const float* temp_eff;    /* host, [steps] */
+  const int32_t* do_sample; /* host, [steps] */
+  uint32_t seed_lo, seed_hi; /* Philox key */
+  float top_p;
+} vnb_gen_group;
+/* n_groups independent VampNet.generate(return_signal=False) calls of the same T and sampling_steps in one launch.
+ * The B batch rows are split into n_groups contiguous groups in order (groups[g].rows each).  Every group keeps what a
+ * call of its own would have: its N0 (the initial mask count over its rows only, transformer.py:766), its temperature,
+ * schedules, top_p and key, and its row numbering (the Philox counter uses the row index within the group).  So
+ * out equals, bit for bit, the concatenation of vnb_generate over each group's rows; vnb_generate is the one-group
+ * case.  gamma: host [steps], shared (it depends on steps only).  z, mask and out as in vnb_generate.
+ * Errors: group rows not summing to B, n_groups < 1 or > B, steps outside 1..256, groups that mix top-p with no top-p
+ * (the sampler variant is per launch).  Graphs are cached per (B, T) workspace as for vnb_generate: the grouping, the
+ * keys and the temperatures are written before every replay and never cause a new capture. */
+int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
+                          int64_t* out, void* stream);
 /* One sampling iteration on caller-supplied logits (B, S, V) fp32 — sample_from_logits +
  * mask_by_random_topk + the where()s around them (transformer.py:849-932).  State is explicit:
  * zflat (B, S) int32 in "t c" order (util.py:39) is updated in place; tokens_out (B, S) int32
@@ -116,7 +138,8 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
  * vnb_launch_count: kernels launched by this library so far in this process (a graph replay adds the
  * number of kernel nodes it contains).
  * vnb_graph_capture_count: generate graphs captured so far (a weight hot swap or a repeated call must not
- * add to it: graphs are cached per (workspace, steps, mask, top_p)).
+ * add to it: graphs are cached per (workspace, steps, mask, top_p); the grouping of vnb_generate_many is not part
+ * of that key).
  * vnb_profile_begin/end: between the two calls every launch of forward/generate is bracketed by CUDA
  * events on the launching stream (graph replay is bypassed so that the events can be recorded);
  * end() returns the summed device time and launch count per kernel family:

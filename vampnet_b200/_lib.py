@@ -38,6 +38,13 @@ class GenParams(C.Structure):
     ]
 
 
+class GenGroup(C.Structure):
+    _fields_ = [
+        ("rows", C.c_int32), ("temperature", C.c_float), ("temp_eff", C.POINTER(C.c_float)),
+        ("do_sample", C.POINTER(C.c_int32)), ("seed_lo", C.c_uint32), ("seed_hi", C.c_uint32), ("top_p", C.c_float),
+    ]
+
+
 _SIGS = {
     "vnb_abi_version": (C.c_int32, []),
     "vnb_last_error": (C.c_char_p, []),
@@ -50,6 +57,9 @@ _SIGS = {
     "vnb_get_hidden": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "vnb_generate": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(GenParams),
                                  C.c_void_p, C.c_void_p]),
+    "vnb_generate_many": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                      C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32, C.c_int32, C.c_void_p,
+                                      C.c_void_p]),
     "vnb_launch_count": (C.c_uint64, []),
     "vnb_graph_capture_count": (C.c_uint64, []),
     "vnb_set_option": (C.c_int32, [C.c_char_p, C.c_int32]),

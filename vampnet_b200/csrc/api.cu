@@ -147,7 +147,10 @@ struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in w
 struct Workspace {
   int B = 0, T = 0, Tpad = 0, M = 0;
   unsigned long long last_use = 0;
-  DevBuf x, y, qk, vT, att, h, logits, zcur, zorig, tokens, conf, n0, dyn, z_in, mask_in, z_out, ssA, ssB, embA, partials;
+  // generate(): n0 (B) = initial mask count per group, dyn (kMaxSteps, B) = the SampleDyn table [step][group] with row
+  // stride B, rowgrp (B) = the group of every batch row; all three are rewritten before every launch or graph replay
+  DevBuf x, y, qk, vT, att, h, logits, zcur, zorig, tokens, conf, n0, dyn, rowgrp, z_in, mask_in, z_out, ssA, ssB, embA,
+      partials;
   int embKp = 0;
   int ss_parts = 0;
   std::vector<GemmPlan> qkv, wo, up, down;
@@ -237,8 +240,9 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   CK(ws->zorig.alloc(M * c.n_codebooks * 4));
   CK(ws->tokens.alloc(M * Cp * 4));
   CK(ws->conf.alloc(M * Cp * 4));
-  CK(ws->n0.alloc(4, true));
-  CK(ws->dyn.alloc(sizeof(SampleDyn) * vnb_model::kMaxSteps));
+  CK(ws->n0.alloc(4 * static_cast<size_t>(B), true));
+  CK(ws->dyn.alloc(sizeof(SampleDyn) * vnb_model::kMaxSteps * B));
+  CK(ws->rowgrp.alloc(sizeof(RowGroup) * B));
   CK(ws->z_in.alloc(M * c.n_codebooks * 8));
   CK(ws->mask_in.alloc(M * c.n_codebooks * 4));
   CK(ws->z_out.alloc(M * c.n_codebooks * 8));
@@ -278,6 +282,7 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
     ws->cls_sample.epi = VNB_EPI_SAMPLE;
     ws->cls_sample.out = nullptr;
     ws->cls_sample.zcur = ws->zcur.as<int32_t>();
+    ws->cls_sample.rowgrp = ws->rowgrp.as<RowGroup>();
     ws->cls_sample.partials = ws->partials.p;
     ws->cls_sample.C = c.n_codebooks; ws->cls_sample.ncc = c.n_conditioning_codebooks;
     ws->cls_sample.V = c.vocab_size; ws->cls_sample.mask_token = c.vocab_size;
@@ -364,6 +369,28 @@ static int stage_sample_dyn(const SampleDyn& d, cudaStream_t st, const SampleDyn
   return 0;
 }
 
+// The row map of a one-call launch of up to `rows` batch rows: all zeros (group 0, starting at row 0).  One buffer per
+// device, grown when a larger batch comes; never written after it is zeroed.
+static int one_group_rows(int rows, const RowGroup** out) {
+  static RowGroup* buf_dev[64] = {nullptr};
+  static int cap_dev[64] = {0};
+  int dev = 0;
+  CK(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return fail("device index %d out of range", dev);
+  if (cap_dev[dev] < rows) {
+    if (buf_dev[dev]) CK(cudaFree(buf_dev[dev]));
+    buf_dev[dev] = nullptr;
+    cap_dev[dev] = 0;
+    const int cap = rows > 1024 ? rows : 1024;
+    CK(cudaMalloc(&buf_dev[dev], sizeof(RowGroup) * cap));
+    CK(cudaMemset(buf_dev[dev], 0, sizeof(RowGroup) * cap));
+    CK(cudaDeviceSynchronize());  // zeroed before any stream of any caller reads it
+    cap_dev[dev] = cap;
+  }
+  *out = buf_dev[dev];
+  return 0;
+}
+
 }  // namespace vnb
 
 using namespace vnb;
@@ -404,8 +431,8 @@ int32_t vnb_forward_codes(vnb_model* m, const int64_t* codes, int32_t B, int32_t
   if (get_workspace(m, B, T, &ws)) return 1;
   const vnb_config& c = m->cfg;
   // (B,C,T) int64 -> (B,T,C) int32, no masking (mask = zeros)
-  LAUNCH(FAM_STATE, launch_gen_init(codes, nullptr, ws->zcur.as<int32_t>(), ws->zorig.as<int32_t>(), ws->n0.as<int32_t>(), B,
-                     c.n_codebooks, T, /*ncc=*/c.n_codebooks, c.vocab_size, st));
+  LAUNCH(FAM_STATE, launch_gen_init(codes, nullptr, ws->zcur.as<int32_t>(), ws->zorig.as<int32_t>(), ws->n0.as<int32_t>(),
+                                    nullptr, 1, B, c.n_codebooks, T, /*ncc=*/c.n_codebooks, c.vocab_size, st));
   if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
   m->last = ws;
   return run_stack(m, ws, logits, st);
@@ -451,8 +478,9 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
                             cudaStream_t st, bool use_top_p, bool fused) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
-  LAUNCH(FAM_STATE, launch_gen_init(z, mask, ws->zcur.as<int32_t>(), ws->zorig.as<int32_t>(), ws->n0.as<int32_t>(), ws->B, c.n_codebooks,
-                     ws->T, ncc, c.vocab_size, st));
+  // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
+  LAUNCH(FAM_STATE, launch_gen_init(z, mask, ws->zcur.as<int32_t>(), ws->zorig.as<int32_t>(), ws->n0.as<int32_t>(),
+                                    ws->rowgrp.as<RowGroup>(), ws->B, ws->B, c.n_codebooks, ws->T, ncc, c.vocab_size, st));
   SampleArgs sa;
   sa.logits = ws->logits.as<float>();
   sa.zcur = ws->zcur.as<int32_t>();
@@ -460,10 +488,11 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   sa.tokens = ws->tokens.as<int32_t>();
   sa.conf = ws->conf.as<float>();
   sa.n0 = ws->n0.as<int32_t>();
+  sa.rowgrp = ws->rowgrp.as<RowGroup>();
   sa.B = ws->B; sa.T = ws->T; sa.C = c.n_codebooks; sa.ncc = ncc; sa.V = c.vocab_size; sa.mask_token = c.vocab_size;
   for (int i = 0; i < steps; ++i) {
     if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
-    const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + i;
+    const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
     if (fused) {
       if (run_stack(m, ws, nullptr, st, nullptr, dyn_i)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
@@ -478,34 +507,56 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   return 0;
 }
 
-int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                     const vnb_gen_params* p, int64_t* out, void* stream) {
+int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
+                          int64_t* out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (!p || p->sampling_steps < 1 || p->sampling_steps > vnb_model::kMaxSteps) return fail("bad sampling_steps");
+  if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
+  if (!gamma || !groups) return fail("vnb_generate_many: gamma and groups are required");
+  if (B < 1 || T < 1) return fail("vnb_generate_many: need B >= 1 and T >= 1 (got %d, %d)", B, T);
+  if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
+  const auto top_p_on = [](float tp) { return tp > 0.f && tp < 1.f; };
+  const bool use_top_p = top_p_on(groups[0].top_p);
+  long long total = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    const vnb_gen_group& q = groups[g];
+    if (q.rows < 1) return fail("vnb_generate_many: group %d has %d rows", g, q.rows);
+    if (!q.temp_eff || !q.do_sample) return fail("vnb_generate_many: group %d lacks its schedules", g);
+    // the sampler variant is chosen per launch: a mixed launch would filter differently from the separate calls
+    if (top_p_on(q.top_p) != use_top_p) return fail("vnb_generate_many: groups mix top-p and no top-p sampling");
+    total += q.rows;
+  }
+  if (total != B) return fail("vnb_generate_many: group rows sum to %lld, not B = %d", total, B);
   Workspace* ws;
   if (get_workspace(m, B, T, &ws)) return 1;
   m->last = ws;
-  const int steps = p->sampling_steps;
-  std::vector<SampleDyn> dyn(steps);
-  const float inv_t = inv_temperature(p->temperature);
-  for (int i = 0; i < steps; ++i) {
-    dyn[i].inv_temp = inv_t;
-    dyn[i].gamma = p->gamma[i];
-    dyn[i].temp_eff = p->temp_eff[i];
-    dyn[i].do_sample = p->do_sample[i];
-    dyn[i].is_last = (i == steps - 1);
-    dyn[i].step = i;
-    dyn[i].seed_lo = p->seed_lo;
-    dyn[i].seed_hi = p->seed_hi;
-    dyn[i].top_p = p->top_p;
+  // the [step][group] table (row stride B) and the row map, pageable sources: the runtime stages them before
+  // returning, so the vectors may die at scope exit
+  std::vector<SampleDyn> dyn(static_cast<size_t>(steps) * B);
+  std::vector<RowGroup> rowgrp(B);
+  for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
+    const vnb_gen_group& q = groups[g];
+    const float inv_t = inv_temperature(q.temperature);
+    for (int i = 0; i < steps; ++i) {
+      SampleDyn& d = dyn[static_cast<size_t>(i) * B + g];
+      d.inv_temp = inv_t;
+      d.gamma = gamma[i];
+      d.temp_eff = q.temp_eff[i];
+      d.do_sample = q.do_sample[i];
+      d.is_last = (i == steps - 1);
+      d.step = i;
+      d.seed_lo = q.seed_lo;
+      d.seed_hi = q.seed_hi;
+      d.top_p = q.top_p;
+    }
+    for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
   }
-  // pageable source: the runtime stages it before returning, so `dyn` may die at scope exit
-  CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * steps, cudaMemcpyHostToDevice, st));
-  const bool use_top_p = p->top_p > 0.f && p->top_p < 1.f;
+  CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * dyn.size(), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
   const bool fused = fused_sampler_enabled() != 0 && !use_top_p && ws->can_fuse;
   if (!fused && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
-  if (!p->use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused);
+  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused);
 
   const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
   CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
@@ -546,6 +597,16 @@ int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_
   g_launches += ws->graph_kernels[key];
   CK(cudaMemcpyAsync(out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// One call is the one-group launch.
+int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                     const vnb_gen_params* p, int64_t* out, void* stream) {
+  if (!p) return fail("bad sampling_steps");
+  vnb_gen_group g;
+  g.rows = B; g.temperature = p->temperature; g.temp_eff = p->temp_eff; g.do_sample = p->do_sample;
+  g.seed_lo = p->seed_lo; g.seed_hi = p->seed_hi; g.top_p = p->top_p;
+  return vnb_generate_many(m, z, mask, B, T, p->sampling_steps, p->gamma, &g, 1, p->use_graph, out, stream);
 }
 
 uint64_t vnb_launch_count(void) { return g_launches; }
@@ -611,9 +672,11 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
   d.gamma = gamma; d.temp_eff = temp_eff; d.do_sample = do_sample; d.is_last = is_last; d.step = step;
   d.seed_lo = seed_lo; d.seed_hi = seed_hi; d.top_p = 0.f;
   const SampleDyn* dd = nullptr;
-  if (stage_sample_dyn(d, st, &dd)) return 1;
+  const RowGroup* rg = nullptr;
+  if (stage_sample_dyn(d, st, &dd) || one_group_rows(B, &rg)) return 1;
   SampleArgs sa;
   sa.logits = logits; sa.zcur = zflat; sa.zorig = nullptr; sa.tokens = tokens_out; sa.conf = conf_out; sa.n0 = n0;
+  sa.rowgrp = rg;
   sa.B = B; sa.T = S; sa.C = 1; sa.ncc = 0; sa.V = V; sa.mask_token = mask_token;
   CK(launch_sample_step_dev(sa, dd, st, false));
   return 0;
@@ -678,7 +741,7 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
     return fail("gemm plan: %s", tmap_error());
   p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
   p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
-  if (stage_sample_dyn(d, st, &p.dyn)) return 1;
+  if (stage_sample_dyn(d, st, &p.dyn) || one_group_rows((M + T - 1) / T, &p.rowgrp)) return 1;
   CK(launch_gemm(p, st));
   return 0;
 }

@@ -63,20 +63,22 @@ cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, 
 
 // ------------------------------------------------------------------------------------------------
 // generate() set-up (reference transformer.py:749-766): z_masked = z.masked_fill(mask, MASK);
-// N0 = count(z_masked == MASK) over the WHOLE batch.  State is kept as (B, T, C) int32 so that the
-// codes of one frame are contiguous for the embedding gather and "b (t c)" flattening (util.py:39)
-// of the predicted codebooks is a plain stride.
+// N0 = count(z_masked == MASK) over the WHOLE batch of one generate() call, i.e. per row group of a launch.  State is
+// kept as (B, T, C) int32 so that the codes of one frame are contiguous for the embedding gather and "b (t c)"
+// flattening (util.py:39) of the predicted codebooks is a plain stride.  blockIdx.y is the batch row, so each block's
+// count belongs to one group.
 __global__ void gen_init_kernel(const int64_t* __restrict__ z, const int32_t* __restrict__ mask,
                                 int32_t* __restrict__ zcur, int32_t* __restrict__ zorig, int32_t* __restrict__ n0,
-                                int B, int C, int T, int ncc, int mask_token) {
-  const int total = B * C * T;
+                                const RowGroup* __restrict__ rowgrp, int C, int T, int ncc, int mask_token) {
+  const int b = blockIdx.y;
+  const int per_row = C * T;
+  const size_t base = static_cast<size_t>(b) * per_row;
   int local = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < per_row; i += gridDim.x * blockDim.x) {
     const int t = i % T;
-    const int c = (i / T) % C;
-    const int b = i / (T * C);
-    const int v = static_cast<int>(z[i]);
-    const int mk = mask ? mask[i] : (c >= ncc ? 1 : 0);  // default mask, transformer.py:749-751
+    const int c = i / T;
+    const int v = static_cast<int>(z[base + i]);
+    const int mk = mask ? mask[base + i] : (c >= ncc ? 1 : 0);  // default mask, transformer.py:749-751
     const int vm = mk ? mask_token : v;
     const size_t o = (static_cast<size_t>(b) * T + t) * C + c;
     zorig[o] = v;
@@ -91,18 +93,20 @@ __global__ void gen_init_kernel(const int64_t* __restrict__ z, const int32_t* __
   if (threadIdx.x < 32) {
     int v = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0;
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (threadIdx.x == 0 && v) atomicAdd(n0, v);
+    if (threadIdx.x == 0 && v) atomicAdd(n0 + (rowgrp ? rowgrp[b].group : 0), v);
   }
 }
 
-cudaError_t launch_gen_init(const int64_t* z, const int32_t* mask, int32_t* zcur, int32_t* zorig, int32_t* n0, int B,
-                            int C, int T, int ncc, int mask_token, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(n0, 0, sizeof(int32_t), st);
+cudaError_t launch_gen_init(const int64_t* z, const int32_t* mask, int32_t* zcur, int32_t* zorig, int32_t* n0,
+                            const RowGroup* rowgrp, int n_groups, int B, int C, int T, int ncc, int mask_token,
+                            cudaStream_t st) {
+  if (B > 65535) return cudaErrorInvalidValue;  // grid y
+  cudaError_t e = cudaMemsetAsync(n0, 0, sizeof(int32_t) * n_groups, st);
   if (e != cudaSuccess) return e;
-  const int total = B * C * T;
-  int grid = (total + 255) / 256;
-  if (grid > 1184) grid = 1184;
-  gen_init_kernel<<<grid, 256, 0, st>>>(z, mask, zcur, zorig, n0, B, C, T, ncc, mask_token);
+  int gx = (C * T + 255) / 256;
+  const int cap = (1184 + B - 1) / B;  // about as many blocks in all as a grid-stride launch of 1184
+  if (gx > cap) gx = cap;
+  gen_init_kernel<<<dim3(gx, B), 256, 0, st>>>(z, mask, zcur, zorig, n0, rowgrp, C, T, ncc, mask_token);
   return cudaGetLastError();
 }
 

@@ -63,7 +63,8 @@ struct GemmArgs {
   float inv_d, eps;         // row scale = rsqrt(sum * inv_d + eps)
   // ---- EPI_SAMPLE (see the epilogue) ----
   const int32_t* zcur;
-  const SampleDyn* dyn;
+  const SampleDyn* dyn;     // this step's row of the (step, group) table
+  const RowGroup* rowgrp;   // (B) group of every batch row
   float4* partials;
   int C, ncc, V, mask_token;
 };
@@ -293,7 +294,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int row = m0 + quad * 32 + lane;
       const bool row_ok = row < g.M;
       int b_idx = 0, t_idx = 0;
-      if constexpr (EPI == VNB_EPI_QKV) {
+      if constexpr (EPI == VNB_EPI_QKV || EPI == VNB_EPI_SAMPLE) {
         b_idx = row / g.T;
         t_idx = row - b_idx * g.T;
       }
@@ -334,8 +335,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (__any_sync(0xffffffffu, active)) {
           const uint32_t t_strip = t_addr + 4u * (strip * 128);
           const uint32_t sb4 = sbias + 4u * (strip * 128);
-          const float inv_temp = g.dyn->inv_temp;
-          const int do_sample = g.dyn->do_sample;
+          // this row's generate() call: its temperature, greedy / sampling step and key, and the row's index in it
+          const RowGroup rg = g.rowgrp[row_ok ? b_idx : 0];
+          const SampleDyn& dyn = g.dyn[rg.group];
+          const float inv_temp = dyn.inv_temp;
+          const int do_sample = dyn.do_sample;
           // sweep 1: maximum and arg-max (lowest index on ties) of the logits
           float mx = -INFINITY;
           int am = 0;
@@ -378,10 +382,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           int cand = am;
           float xc = mx;
           if (do_sample) {
-            const int b_idx = row / g.T, t_idx = row - b_idx * g.T;
             uint32_t r4[4];
-            philox4x32_10(static_cast<uint32_t>(t_idx * Cp + cp), static_cast<uint32_t>(b_idx),
-                          static_cast<uint32_t>(g.dyn->step), 0u, g.dyn->seed_lo, g.dyn->seed_hi, r4);
+            philox4x32_10(static_cast<uint32_t>(t_idx * Cp + cp), static_cast<uint32_t>(b_idx - rg.first),
+                          static_cast<uint32_t>(dyn.step), 0u, dyn.seed_lo, dyn.seed_hi, r4);
             const float target = u01(r4[1]) * ssum;
             float run = 0.f;
             int found = -1;
@@ -562,7 +565,7 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
   g.T = p.T; g.Tpad = p.Tpad; g.d2 = p.d2;
   g.out_bf16 = reinterpret_cast<__nv_bfloat16*>(p.out_bf16); g.ss_out = p.ss_out; g.ss_in = p.ss_in;
   g.ss_parts = p.ss_parts; g.inv_d = p.inv_d; g.eps = p.eps;
-  g.zcur = p.zcur; g.dyn = p.dyn; g.partials = reinterpret_cast<float4*>(p.partials);
+  g.zcur = p.zcur; g.dyn = p.dyn; g.rowgrp = p.rowgrp; g.partials = reinterpret_cast<float4*>(p.partials);
   g.C = p.C; g.ncc = p.ncc; g.V = p.V; g.mask_token = p.mask_token;
   switch (p.epi) {
     case VNB_EPI_BF16: return launch_epi<VNB_EPI_BF16>(p, g, st);
@@ -571,7 +574,7 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
     case VNB_EPI_GEGLU: return launch_epi<VNB_EPI_GEGLU>(p, g, st);
     case VNB_EPI_BIAS_F32: return launch_epi<VNB_EPI_BIAS_F32>(p, g, st);
     case VNB_EPI_SAMPLE:
-      if (!p.zcur || !p.dyn || !p.partials || !p.bias || p.V % 128 != 0 || p.V > 1024) return cudaErrorInvalidValue;
+      if (!p.zcur || !p.dyn || !p.rowgrp || !p.partials || !p.bias || p.V % 128 != 0 || p.V > 1024) return cudaErrorInvalidValue;
       return launch_epi<VNB_EPI_SAMPLE>(p, g, st);
     default: return cudaErrorInvalidValue;
   }

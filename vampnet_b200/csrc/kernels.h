@@ -45,6 +45,10 @@ extern "C" int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 namespace vnb {
 
 struct SampleDyn;
+// Batch row b of a generate launch belongs to group `group` (one would-be generate() call) whose rows start at `first`.
+struct RowGroup {
+  int32_t group, first;
+};
 
 // ---- GEMM ----
 struct GemmPlan {
@@ -63,7 +67,8 @@ struct GemmPlan {
   float inv_d = 0.f, eps = 0.f;
   // VNB_EPI_SAMPLE (the classifier of the generate loop): the logits are sampled in the epilogue instead of being stored
   const int32_t* zcur = nullptr;     // (B, T, C) current tokens: only still-masked positions are sampled
-  const SampleDyn* dyn = nullptr;    // this step's scalars (device memory: graph replay safe)
+  const SampleDyn* dyn = nullptr;    // this step's scalars, one per group (device memory: graph replay safe)
+  const RowGroup* rowgrp = nullptr;  // (B) group of every batch row
   void* partials = nullptr;          // (M * Cp * V/128) float4 records, see sample_combine_kernel
   int C = 0, ncc = 0, V = 0, mask_token = 0;
 };
@@ -98,16 +103,19 @@ cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, 
                                 int C, int V1, int K, int Kp, float* ss, int zero_from, int ss_parts, cudaStream_t st);
 
 // ---- generate-loop state kernels ----
-// z (B,C,T) int64, mask (B,C,T) int32|null -> zcur (B,T,C) int32 (masked), zorig (B,T,C) int32; n0 += count(MASK)
-cudaError_t launch_gen_init(const int64_t* z, const int32_t* mask, int32_t* zcur, int32_t* zorig, int32_t* n0, int B,
-                            int C, int T, int ncc, int mask_token, cudaStream_t st);
+// z (B,C,T) int64, mask (B,C,T) int32|null -> zcur (B,T,C) int32 (masked), zorig (B,T,C) int32;
+// n0[g] = count(MASK) over the rows of group g (rowgrp null: every row is in group 0), n0 zeroed first for g < n_groups
+cudaError_t launch_gen_init(const int64_t* z, const int32_t* mask, int32_t* zcur, int32_t* zorig, int32_t* n0,
+                            const RowGroup* rowgrp, int n_groups, int B, int C, int T, int ncc, int mask_token,
+                            cudaStream_t st);
 // tokens (B, T, Cp) int32 + zorig cond -> out (B, C, T) int64
 cudaError_t launch_gen_finish(const int32_t* tokens, const int32_t* zorig, int64_t* out, int B, int C, int T, int ncc,
                               cudaStream_t st);
 
-// per-step dynamic scalars, read from DEVICE memory so that a captured CUDA graph can be replayed with
-// new temperatures / seeds (the schedule values are computed on the host with the reference's fp32
-// expressions: mask.py:8-9, transformer.py:831-834, 917-919)
+// per-(step, group) dynamic scalars, read from DEVICE memory so that a captured CUDA graph can be replayed with
+// new groupings / temperatures / seeds (the schedule values are computed on the host with the reference's fp32
+// expressions: mask.py:8-9, transformer.py:831-834, 917-919).  The sampling kernels take a step's row of the table
+// and read entry rowgrp[b].group for batch row b.
 struct SampleDyn {
   float inv_temp, gamma, temp_eff;
   int do_sample, is_last, step;
@@ -120,7 +128,8 @@ struct SampleArgs {
   const int32_t* zorig; // (B, T, C) int32 or null (then conditioning codebooks are left untouched)
   int32_t* tokens;      // (B, T, Cp) sampled_z
   float* conf;          // (B, S)
-  const int32_t* n0;    // device scalar
+  const int32_t* n0;    // (groups) initial mask count of each group
+  const RowGroup* rowgrp;  // (B)
   int B, T, C, ncc, V, mask_token;
 };
 // use_top_p selects the kernel variant at launch time (it is baked into a captured graph: part of the graph key)

@@ -36,19 +36,22 @@ struct SampleStatic {
   int32_t* tokens;
   float* conf;
   const int32_t* n0;
+  const RowGroup* rowgrp;
   int B, T, C, ncc, V, mask_token;
 };
 
 // TOPP = false compiles the nucleus filter out (its 32 extra live registers cost occupancy on the common path)
 template <bool TOPP>
 __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const SampleStatic a, const SampleDynDev* __restrict__ dynp) {
-  const SampleDynDev dyn = *dynp;
   const int Cp = a.C - a.ncc;
   const int S = a.T * Cp;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= a.B * S) return;
   const int lane = threadIdx.x & 31;
   const int b = row / S, s = row - b * S;
+  const RowGroup rg = a.rowgrp[b];
+  const SampleDynDev dyn = dynp[rg.group];
+  const uint32_t bg = static_cast<uint32_t>(b - rg.first);  // Philox counter word: the row within its own call
   const int t = s / Cp, cp = s - t * Cp;
   const int zi = a.zcur[(static_cast<size_t>(b) * a.T + t) * a.C + a.ncc + cp];
   if (zi != a.mask_token) {  // known token: kept, never re-masked (transformer.py:893-900)
@@ -161,8 +164,7 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
   }
   if (dyn.do_sample) {
     uint32_t r[4];
-    philox4x32_10(static_cast<uint32_t>(s), static_cast<uint32_t>(b), static_cast<uint32_t>(dyn.step), 0u, dyn.seed_lo,
-                  dyn.seed_hi, r);
+    philox4x32_10(static_cast<uint32_t>(s), bg, static_cast<uint32_t>(dyn.step), 0u, dyn.seed_lo, dyn.seed_hi, r);
     // Two-level inverse CDF (oracle/vampnet_oracle.py sample_from_logits, rng="philox"): uniform 1 picks the
     // 128-entry tile (= chunk i of this layout) by its mass, uniform 2 the entry inside it.  The classifier GEMM's
     // sampling epilogue (gemm_wgmma.cu, EPI_SAMPLE) draws the same way from its own 128-column strips.
@@ -234,8 +236,7 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
   if (lane == 0) {
     const float p = expf(xt - m) / se;
     uint32_t r[4];
-    philox4x32_10(static_cast<uint32_t>(s), static_cast<uint32_t>(b), static_cast<uint32_t>(dyn.step), 1u, dyn.seed_lo,
-                  dyn.seed_hi, r);
+    philox4x32_10(static_cast<uint32_t>(s), bg, static_cast<uint32_t>(dyn.step), 1u, dyn.seed_lo, dyn.seed_hi, r);
     // confidence = log p + temperature * Gumbel (transformer.py:1055-1057)
     const float cf = __fadd_rn(logf(p), __fmul_rn(dyn.temp_eff, gumbel(u01(r[0]))));
     a.tokens[row] = best_i;
@@ -244,10 +245,11 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
 }
 
 __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, const SampleDynDev* __restrict__ dynp) {
-  const SampleDynDev dyn = *dynp;
   const int Cp = a.C - a.ncc;
   const int S = a.T * Cp;
   const int b = blockIdx.x;
+  const int grp = a.rowgrp[b].group;
+  const SampleDynDev dyn = dynp[grp];
   const float* conf = a.conf + static_cast<size_t>(b) * S;
   const int32_t* tok = a.tokens + static_cast<size_t>(b) * S;
   int32_t* zrow = a.zcur + static_cast<size_t>(b) * a.T * a.C;
@@ -267,8 +269,8 @@ __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, cons
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(&s_cnt, local);
   __syncthreads();
   if (threadIdx.x == 0) {
-    // num_to_mask = floor(gamma(r) * N0) in fp32 (transformer.py:903), clamped unless last step
-    int n = static_cast<int>(floorf(__fmul_rn(dyn.gamma, static_cast<float>(*a.n0))));
+    // num_to_mask = floor(gamma(r) * N0) in fp32 (transformer.py:903), N0 of this row's call, clamped unless last step
+    int n = static_cast<int>(floorf(__fmul_rn(dyn.gamma, static_cast<float>(a.n0[grp]))));
     if (!dyn.is_last) {
       int up = s_cnt - 1;
       if (n > up) n = up;
@@ -330,12 +332,14 @@ __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, cons
 // never reach HBM.  Algorithmic bytes: 16 * V/128 per masked row.
 __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic a, const float4* __restrict__ partials,
                                                              const SampleDynDev* __restrict__ dynp) {
-  const SampleDynDev dyn = *dynp;
   const int Cp = a.C - a.ncc;
   const int S = a.T * Cp;
   const int row = blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= a.B * S) return;
   const int b = row / S, s = row - b * S;
+  const RowGroup rg = a.rowgrp[b];
+  const SampleDynDev dyn = dynp[rg.group];
+  const uint32_t bg = static_cast<uint32_t>(b - rg.first);
   const int t = s / Cp, cp = s - t * Cp;
   const int zi = a.zcur[(static_cast<size_t>(b) * a.T + t) * a.C + a.ncc + cp];
   if (zi != a.mask_token) {  // known token: kept, never re-masked (transformer.py:893-900)
@@ -368,8 +372,7 @@ __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic 
   int kk = kmax;
   if (dyn.do_sample) {
     uint32_t r[4];
-    philox4x32_10(static_cast<uint32_t>(s), static_cast<uint32_t>(b), static_cast<uint32_t>(dyn.step), 0u, dyn.seed_lo,
-                  dyn.seed_hi, r);
+    philox4x32_10(static_cast<uint32_t>(s), bg, static_cast<uint32_t>(dyn.step), 0u, dyn.seed_lo, dyn.seed_hi, r);
     const float target = u01(r[0]) * total;
     float run = 0.f;
     int pick = -1;
@@ -390,8 +393,7 @@ __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic 
   const int token = dyn.do_sample ? static_cast<int>(bits & 0xffffu) : static_cast<int>(bits >> 16);
   const float p = fast_exp2(__fmul_rn(xc - M, c1)) / total;
   uint32_t r[4];
-  philox4x32_10(static_cast<uint32_t>(s), static_cast<uint32_t>(b), static_cast<uint32_t>(dyn.step), 1u, dyn.seed_lo,
-                dyn.seed_hi, r);
+  philox4x32_10(static_cast<uint32_t>(s), bg, static_cast<uint32_t>(dyn.step), 1u, dyn.seed_lo, dyn.seed_hi, r);
   a.tokens[row] = token;
   a.conf[row] = __fadd_rn(logf(p), __fmul_rn(dyn.temp_eff, gumbel(u01(r[0]))));
 }
@@ -399,6 +401,7 @@ __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic 
 static SampleStatic make_static(const SampleArgs& s) {
   SampleStatic a;
   a.logits = s.logits; a.zcur = s.zcur; a.zorig = s.zorig; a.tokens = s.tokens; a.conf = s.conf; a.n0 = s.n0;
+  a.rowgrp = s.rowgrp;
   a.B = s.B; a.T = s.T; a.C = s.C; a.ncc = s.ncc; a.V = s.V; a.mask_token = s.mask_token;
   return a;
 }

@@ -199,11 +199,9 @@ class Interface(torch.nn.Module):
         return [(lo, min(lo + span, total)) for lo in range(0, total, span)]
 
     # ------------------------------------------------------------------ coarse -> fine (interface.py:327-380)
-    @torch.inference_mode()
-    def coarse_to_fine(self, z: torch.Tensor, mask: torch.Tensor = None, return_mask: bool = False, **kwargs):
-        """Fill the fine codebooks given the coarse ones, c2f.chunk_size_s seconds at a time.  The sequence is
-        zero-padded to a whole number of chunks (padding frames masked), missing codebooks are appended as zeros and
-        the conditioning codebooks are never masked; every chunk is an independent generate() call."""
+    def _c2f_plan(self, z: torch.Tensor, mask: torch.Tensor = None):
+        """The chunks of coarse_to_fine: the generate() arguments of each chunk (time_steps, start_tokens, mask) and
+        the state _c2f_stitch needs."""
         assert self.c2f is not None, "No coarse2fine model loaded"
         n_frames = z.shape[-1]
         span = self.s2t(self.c2f.chunk_size_s)
@@ -218,11 +216,12 @@ class Interface(torch.nn.Module):
         if mask is not None:
             mask = mask.clone()
             mask[:, :self.c2f.n_conditioning_codebooks, :] = 0
-        parts = []
-        for lo, hi in self._spans(z.shape[-1], span):
-            parts.append(self.c2f.generate(codec=self.codec, time_steps=span, start_tokens=z[..., lo:hi],
-                                           mask=None if mask is None else mask[..., lo:hi], return_signal=False,
-                                           cfg_guidance=None, **kwargs))
+        chunks = [dict(time_steps=span, start_tokens=z[..., lo:hi], mask=None if mask is None else mask[..., lo:hi])
+                  for lo, hi in self._spans(z.shape[-1], span)]
+        return chunks, (n_frames, mask)
+
+    def _c2f_stitch(self, parts: list, state, return_mask: bool):
+        n_frames, mask = state
         fine = torch.cat(parts, dim=-1)
         result = fine[..., :n_frames].clone()
         if not return_mask:
@@ -230,19 +229,25 @@ class Interface(torch.nn.Module):
         remasked, _ = pmask.apply_mask(fine, mask, self.c2f.mask_token)
         return result, remasked[..., :n_frames].clone()
 
-    # ------------------------------------------------------------------ coarse (interface.py:382-452)
     @torch.inference_mode()
-    def coarse_vamp(self, z, mask, return_mask=False, gen_fn=None, **kwargs):
-        """Regenerate the masked coarse tokens, coarse.chunk_size_s seconds at a time.  A chunk that keeps at least one
-        frame also keeps its first and last frame as anchors so that stitched chunks do not jump
-        (interface.py:407-413).  Fine codebooks ride along untouched."""
+    def coarse_to_fine(self, z: torch.Tensor, mask: torch.Tensor = None, return_mask: bool = False, **kwargs):
+        """Fill the fine codebooks given the coarse ones, c2f.chunk_size_s seconds at a time.  The sequence is
+        zero-padded to a whole number of chunks (padding frames masked), missing codebooks are appended as zeros and
+        the conditioning codebooks are never masked; every chunk is an independent generate() call."""
+        chunks, state = self._c2f_plan(z, mask)
+        parts = [self.c2f.generate(codec=self.codec, **c, return_signal=False, cfg_guidance=None, **kwargs)
+                 for c in chunks]
+        return self._c2f_stitch(parts, state, return_mask)
+
+    # ------------------------------------------------------------------ coarse (interface.py:382-452)
+    def _coarse_plan(self, z, mask):
+        """The chunks of coarse_vamp: the generate() arguments of each chunk (time_steps, start_tokens, mask)."""
         n_books = self.coarse.n_codebooks
         tokens, keep = z[:, :n_books, :].clone(), mask[:, :n_books, :]
         assert keep.dtype == torch.long, f"mask must be long dtype, but got {keep.dtype}"
         assert bool(((keep == 0) | (keep == 1)).all()), "mask must be binary"   # the one host sync of this call
         span = self.s2t(self.coarse.chunk_size_s)
-        run = gen_fn or self.coarse.generate
-        starts, results = [], []
+        chunks = []
         for lo, hi in self._spans(tokens.shape[-1], span):
             # a chunk that keeps anything also keeps its first and last frame; decided on the device (no sync):
             # edge value = 0 where any(m == 0) else unchanged
@@ -251,11 +256,22 @@ class Interface(torch.nn.Module):
             m[..., 0] = torch.where(anchors, torch.zeros_like(m[..., 0]), m[..., 0])
             m[..., -1] = torch.where(anchors, torch.zeros_like(m[..., -1]), m[..., -1])
             start, m = pmask.apply_mask(tokens[..., lo:hi], m, self.coarse.mask_token, check=False)
-            starts.append(start)
-            results.append(run(codec=self.codec, time_steps=span, start_tokens=start, mask=m, return_signal=False,
-                               **kwargs))
-        out = torch.cat([torch.cat(results, dim=-1), z[:, n_books:, :]], dim=1)
-        return (out, torch.cat(starts, dim=-1)) if return_mask else out
+            chunks.append(dict(time_steps=span, start_tokens=start, mask=m))
+        return chunks
+
+    def _coarse_stitch(self, z, chunks: list, results: list, return_mask: bool):
+        out = torch.cat([torch.cat(results, dim=-1), z[:, self.coarse.n_codebooks:, :]], dim=1)
+        return (out, torch.cat([c["start_tokens"] for c in chunks], dim=-1)) if return_mask else out
+
+    @torch.inference_mode()
+    def coarse_vamp(self, z, mask, return_mask=False, gen_fn=None, **kwargs):
+        """Regenerate the masked coarse tokens, coarse.chunk_size_s seconds at a time.  A chunk that keeps at least one
+        frame also keeps its first and last frame as anchors so that stitched chunks do not jump
+        (interface.py:407-413).  Fine codebooks ride along untouched."""
+        chunks = self._coarse_plan(z, mask)
+        run = gen_fn or self.coarse.generate
+        results = [run(codec=self.codec, **c, return_signal=False, **kwargs) for c in chunks]
+        return self._coarse_stitch(z, chunks, results, return_mask)
 
     # ------------------------------------------------------------------ masks (interface.py:454-489)
     def build_mask(self, z: torch.Tensor, sig: AudioSignal = None, rand_mask_intensity: float = 1.0,
@@ -280,11 +296,8 @@ class Interface(torch.nn.Module):
         return pmask.codebook_mask(mask, int(upper_codebook_mask), None)
 
     # ------------------------------------------------------------------ vamp (interface.py:491-562)
-    def vamp(self, codes: torch.Tensor, mask: torch.Tensor, batch_size: int = 1, feedback_steps: int = 1,
-             time_stretch_factor: int = 1, return_mask: bool = False, **kwargs):
-        """codes, mask (1|B, 14, T) -> (B, 14, T'): coarse stage (`feedback_steps` passes, kwargs forwarded to
-        generate) then the fine stage, which the reference pins to 2 sampling steps with default temperature
-        (interface.py:545-551).  time_stretch_factor k > 1 inserts k-1 always-masked frames after every frame."""
+    @staticmethod
+    def _vamp_inputs(codes, mask, batch_size: int, time_stretch_factor: int):
         z = codes.expand(batch_size, -1, -1)
         mask = mask.expand(batch_size, -1, -1)
         k = int(time_stretch_factor)
@@ -293,14 +306,80 @@ class Interface(torch.nn.Module):
             inserted = torch.ones_like(z)
             inserted[..., ::k] = 0
             mask = (mask.repeat_interleave(k, dim=-1).bool() | inserted.bool()).long()
+        return z, mask
+
+    def _vamp_result(self, z, zv, coarse_start, fine_start, return_mask: bool):
+        if not return_mask:
+            return zv
         n_coarse = self.coarse.n_codebooks
+        return zv, torch.cat([coarse_start[:, :n_coarse, :], fine_start[:, n_coarse:, :]], dim=1).cpu()
+
+    def _with_fine_books(self, z, zv):
+        """The coarse stage's output with the input's fine codebooks re-attached when the coarse model lacks them."""
+        return torch.cat([zv, z[:, self.coarse.n_codebooks:, :]], dim=1) if zv.shape[1] < z.shape[1] else zv
+
+    # the fine stage's generate arguments, pinned by the reference (interface.py:545-551)
+    _C2F_KWARGS = dict(typical_filtering=True, _sampling_steps=2)
+
+    def vamp(self, codes: torch.Tensor, mask: torch.Tensor, batch_size: int = 1, feedback_steps: int = 1,
+             time_stretch_factor: int = 1, return_mask: bool = False, **kwargs):
+        """codes, mask (1|B, 14, T) -> (B, 14, T'): coarse stage (`feedback_steps` passes, kwargs forwarded to
+        generate) then the fine stage, which the reference pins to 2 sampling steps with default temperature
+        (interface.py:545-551).  time_stretch_factor k > 1 inserts k-1 always-masked frames after every frame."""
+        z, mask = self._vamp_inputs(codes, mask, batch_size, time_stretch_factor)
         zv = z
         for i in range(feedback_steps):
             zv, coarse_start = self.coarse_vamp(zv, mask=mask, return_mask=True, **kwargs)
             coarse_start = coarse_start.roll(shifts=(i + 1) % feedback_steps, dims=-1)
-        if zv.shape[1] < z.shape[1]:
-            zv = torch.cat([zv, z[:, n_coarse:, :]], dim=1)
-        zv, fine_start = self.coarse_to_fine(zv, mask=mask, typical_filtering=True, _sampling_steps=2, return_mask=True)
-        if not return_mask:
-            return zv
-        return zv, torch.cat([coarse_start[:, :n_coarse, :], fine_start[:, n_coarse:, :]], dim=1).cpu()
+        zv, fine_start = self.coarse_to_fine(self._with_fine_books(z, zv), mask=mask, return_mask=True,
+                                             **self._C2F_KWARGS)
+        return self._vamp_result(z, zv, coarse_start, fine_start, return_mask)
+
+    @torch.inference_mode()
+    def vamp_many(self, requests: list):
+        """Serve many vamp() calls together.  Each request is a dict of vamp() arguments (codes, mask, and optionally
+        batch_size, feedback_steps, time_stretch_factor, return_mask and generate keyword arguments).  Returns the
+        list the sequential vamp() calls return, bit for bit, and leaves the random, numpy and torch RNG states as
+        they would: every chunk's key is drawn first, in the sequential calls' order.
+
+        The requests advance stage by stage: feedback pass i runs the chunks of every request that has a pass i as
+        one generate_many(), then the fine stage runs every request's chunks as one more.  Chunks of equal length,
+        within a request or across requests, so share launches."""
+        from .modules.transformer import draw_philox_key
+        reqs = []
+        for r in requests:
+            r = dict(r)
+            q = dict(codes=r.pop("codes"), mask=r.pop("mask"), batch_size=r.pop("batch_size", 1),
+                      feedback_steps=r.pop("feedback_steps", 1), time_stretch_factor=r.pop("time_stretch_factor", 1),
+                      return_mask=r.pop("return_mask", False))
+            q["z"], q["mask"] = self._vamp_inputs(q["codes"], q["mask"], q["batch_size"], q["time_stretch_factor"])
+            q["zv"] = q["z"]
+            seed, key = r.pop("seed", None), r.pop("philox_key", None)
+            q["gen"] = r
+
+            def keys(n, seed=seed, key=key):
+                return [key if key is not None else draw_philox_key(seed) for _ in range(n)]
+            # what the sequential vamp() draws: each coarse pass's chunks, then the fine stage's chunks
+            n_frames = q["z"].shape[-1]
+            n_coarse = len(self._spans(n_frames, self.s2t(self.coarse.chunk_size_s)))
+            q["keys"] = [keys(n_coarse) for _ in range(q["feedback_steps"])]
+            q["c2f_keys"] = [draw_philox_key(None) for _ in self._spans(n_frames, self.s2t(self.c2f.chunk_size_s))]
+            reqs.append(q)
+        for i in range(max((q["feedback_steps"] for q in reqs), default=0)):
+            stage = [q for q in reqs if q["feedback_steps"] > i]
+            plans = [self._coarse_plan(q["zv"], q["mask"]) for q in stage]
+            calls = [dict(**c, return_signal=False, philox_key=k, **q["gen"])
+                     for q, plan in zip(stage, plans) for c, k in zip(plan, q["keys"][i])]
+            results = iter(self.coarse.generate_many(self.codec, calls))
+            for q, plan in zip(stage, plans):
+                q["zv"], start = self._coarse_stitch(q["zv"], plan, [next(results) for _ in plan], True)
+                q["coarse_start"] = start.roll(shifts=(i + 1) % q["feedback_steps"], dims=-1)
+        plans = [self._c2f_plan(self._with_fine_books(q["z"], q["zv"]), q["mask"]) for q in reqs]
+        calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **self._C2F_KWARGS)
+                 for q, (chunks, _) in zip(reqs, plans) for c, k in zip(chunks, q["c2f_keys"])]
+        results = iter(self.c2f.generate_many(self.codec, calls))
+        out = []
+        for q, (chunks, state) in zip(reqs, plans):
+            zv, fine_start = self._c2f_stitch([next(results) for _ in chunks], state, True)
+            out.append(self._vamp_result(q["z"], zv, q.get("coarse_start"), fine_start, q["return_mask"]))
+        return out

@@ -170,6 +170,24 @@ def gamma_schedule(steps: int):
     return r, g
 
 
+def draw_philox_key(seed=None) -> int:
+    """The sampler's 64-bit Philox key of one generate() call.  A seed reseeds random, numpy and torch (at.util.seed,
+    reference transformer.py:711), a process-global side effect callers rely on, and is the key; without a seed the key
+    is drawn from torch's (possibly user-seeded) global generator.  Batched callers draw their keys with this in the
+    order the sequential calls would, so keys and RNG state afterwards are the same."""
+    if seed is not None:
+        random.seed(seed)
+        np.random.seed(seed)
+        torch.manual_seed(seed)
+        return int(seed) & 0xFFFFFFFFFFFFFFFF
+    return int(torch.randint(0, 2 ** 62, (1,)).item())
+
+
+# generate_many() splits a launch whose B*T would exceed this many rows: M = 24576 is the largest GEMM height the
+# benchmarks measure (BASELINE.json configs[4], B = 8 at T = 3072)
+MANY_MAX_ROWS = 24576
+
+
 class VampNet(nn.Module):
     def __init__(
         self,
@@ -478,6 +496,7 @@ class VampNet(nn.Module):
         cfg_scale: float = 3.0,
         cfg_guidance: float = None,
         cond=None,
+        philox_key: int = None,
     ):
         """Iterative parallel decoding, reference transformer.py:686-946.
 
@@ -485,18 +504,58 @@ class VampNet(nn.Module):
         typical_mass / typical_min_tokens (its result is discarded at :989-993), causal_weight, cond,
         cfg_scale, debug.  cfg_guidance only computes an unused tensor in the reference (:845-847) but also
         doubles the batch; it is None on every call path of Interface and is rejected here.
+        philox_key (not in the reference): a key already drawn with draw_philox_key(); the global RNGs are then left
+        alone, and `seed` must be None.
         """
+        call = self._prepare_call(codec, time_steps, _sampling_steps, start_tokens, temperature, mask,
+                                  mask_temperature, ctrls, ctrl_masks, top_p, seed, sample_cutoff, cfg_guidance,
+                                  philox_key)
+        out = self._launch_calls([call])[0]
+        if return_signal:
+            return self.decode(out, codec)
+        return out
+
+    @torch.inference_mode()
+    def generate_many(self, codec, calls):
+        """Run many independent generate() calls, batched into as few launches as the shapes allow.
+
+        `calls` is a list of dicts of generate() keyword arguments.  The result equals
+        [self.generate(codec, **c) for c in calls] bit for bit, return_signal included, and the random, numpy and torch
+        global RNG states afterwards are those the sequential calls leave: keys are drawn (draw_philox_key) in list
+        order.  Calls with the same T, sampling steps and top-p on/off share one vnb_generate_many launch, in which
+        each keeps its own N0, temperatures, schedules, top_p and key; a launch whose B*T would exceed MANY_MAX_ROWS is
+        split."""
+        import inspect
+        sig = inspect.signature(VampNet.generate)
+        prepared, want_signal = [], []
+        for kw in calls:
+            a = sig.bind(self, codec, **kw)
+            a.apply_defaults()
+            a = a.arguments
+            prepared.append(self._prepare_call(codec, a["time_steps"], a["_sampling_steps"], a["start_tokens"],
+                                               a["temperature"], a["mask"], a["mask_temperature"], a["ctrls"],
+                                               a["ctrl_masks"], a["top_p"], a["seed"], a["sample_cutoff"],
+                                               a["cfg_guidance"], a["philox_key"]))
+            want_signal.append(bool(a["return_signal"]))
+        outs = self._launch_calls(prepared)
+        return [self.decode(o, codec) if sig_ else o for o, sig_ in zip(outs, want_signal)]
+
+    def _prepare_call(self, codec, time_steps, steps, start_tokens, temperature, mask, mask_temperature, ctrls,
+                      ctrl_masks, top_p, seed, sample_cutoff, cfg_guidance, philox_key) -> dict:
+        """Validate one generate() call, draw its key and stage its device inputs and per-step host schedules."""
         if ctrls is not None or ctrl_masks is not None:
             raise NotImplementedError("ctrls/ctrl_masks: ControlEncoder is outside the hot path")
         if cfg_guidance is not None:
             raise NotImplementedError("cfg_guidance is dead code in the reference (transformer.py:845-847)")
-        if seed is not None:  # at.util.seed(seed): process-global side effect callers rely on (transformer.py:711)
-            random.seed(seed)
-            np.random.seed(seed)
-            torch.manual_seed(seed)
+        if philox_key is not None:
+            if seed is not None:
+                raise ValueError("generate: pass either seed or philox_key, not both")
+            k = int(philox_key) & 0xFFFFFFFFFFFFFFFF
+        else:
+            k = draw_philox_key(seed)
         self._ensure_handle(codec)
         dev = self.device
-        steps = int(_sampling_steps)
+        steps = int(steps)
         if start_tokens is None:
             z = torch.full((1, self.n_codebooks, time_steps), self.mask_token, device=dev, dtype=torch.int64)
         else:
@@ -509,27 +568,72 @@ class VampNet(nn.Module):
                 mask = mask[:, None, :].repeat(1, C_, 1)
             # the reference applies the mask with z.masked_fill(mask.bool(), ...) (:762): broadcastable masks are legal
             m32 = (mask.to(dev) != 0).expand_as(z).to(torch.int32).contiguous()
-        # Philox key: from the seed when given, else from torch's (possibly user-seeded) global generator
-        if seed is not None:
-            k = int(seed) & 0xFFFFFFFFFFFFFFFF
-        else:
-            k = int(torch.randint(0, 2 ** 62, (1,)).item())
         r, g = gamma_schedule(steps)
         temp_eff = (mask_temperature * (1 - r)).to(torch.float32)
-        gam = (C.c_float * steps)(*[float(v) for v in g])
-        tef = (C.c_float * steps)(*[float(v) for v in temp_eff])
-        dos = (C.c_int32 * steps)(*[1 if (i / steps) <= sample_cutoff else 0 for i in range(steps)])
-        gp = _lib.GenParams(steps, float(temperature), gam, tef, dos, k & 0xFFFFFFFF, (k >> 32) & 0xFFFFFFFF,
-                            1 if self.use_cuda_graph else 0, float(top_p) if (top_p is not None and top_p < 1.0) else 0.0)
+        return dict(z=z, mask=m32, steps=steps, temperature=float(temperature), gamma=[float(v) for v in g],
+                    temp_eff=[float(v) for v in temp_eff],
+                    do_sample=[1 if (i / steps) <= sample_cutoff else 0 for i in range(steps)], key=k,
+                    top_p=float(top_p) if (top_p is not None and top_p < 1.0) else 0.0)
+
+    def _launch_calls(self, calls: list) -> list:
+        """Launch prepared calls, one vnb_generate_many per (T, steps, top-p on) bucket of at most MANY_MAX_ROWS rows
+        (a single larger call runs alone); returns each call's (B, C, T) int64 tokens in list order."""
+        buckets = {}
+        for i, c in enumerate(calls):
+            top_p_on = 0.0 < c["top_p"] < 1.0
+            buckets.setdefault((c["z"].shape[-1], c["steps"], top_p_on), []).append(i)
+        launches = []
+        for (T, _, _), idx in buckets.items():
+            cur, rows = [], 0
+            for i in idx:
+                B = calls[i]["z"].shape[0]
+                if cur and (rows + B) * T > MANY_MAX_ROWS:
+                    launches.append(cur)
+                    cur, rows = [], 0
+                cur.append(i)
+                rows += B
+            launches.append(cur)
+        outs = [None] * len(calls)
+        keep = []
+        for idx in launches:
+            group = [calls[i] for i in idx]
+            for i, o in zip(idx, self._launch_group(group, keep)):
+                outs[i] = o
+        # graph replay bakes the input pointers: keep them alive until the stream has consumed them
+        self._last_io = keep
+        return outs
+
+    def _launch_group(self, calls: list, keep: list) -> list:
+        dev = self.device
+        if len(calls) == 1:
+            z, m32 = calls[0]["z"], calls[0]["mask"]
+        else:
+            z = torch.cat([c["z"] for c in calls])
+            m32 = None
+            if any(c["mask"] is not None for c in calls):
+                # a call without a mask gets the default one materialised (predicted codebooks masked,
+                # transformer.py:749-751): the launch takes one mask for all rows
+                default = (torch.arange(self.n_codebooks, device=dev) >= self.n_conditioning_codebooks).to(torch.int32)
+                m32 = torch.cat([c["mask"] if c["mask"] is not None else default[None, :, None].expand_as(c["z"])
+                                 for c in calls]).contiguous()
+        B, _, T = z.shape
+        steps = calls[0]["steps"]
+        arrays = []
+        groups = (_lib.GenGroup * len(calls))()
+        for g, c in zip(groups, calls):
+            tef = (C.c_float * steps)(*c["temp_eff"])
+            dos = (C.c_int32 * steps)(*c["do_sample"])
+            arrays += [tef, dos]
+            g.rows, g.temperature, g.temp_eff, g.do_sample = c["z"].shape[0], c["temperature"], tef, dos
+            g.seed_lo, g.seed_hi, g.top_p = c["key"] & 0xFFFFFFFF, (c["key"] >> 32) & 0xFFFFFFFF, c["top_p"]
+        gam = (C.c_float * steps)(*calls[0]["gamma"])
         out = torch.empty_like(z)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().vnb_generate(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, C.byref(gp),
-                                               _lib.ptr(out), _lib.stream_ptr(dev)))
-        # graph replay bakes the input pointers: keep them alive until the stream has consumed them
-        self._last_io = (z, m32, out)
-        if return_signal:
-            return self.decode(out, codec)
-        return out
+            _lib.check(_lib.lib().vnb_generate_many(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam, groups,
+                                                    len(calls), 1 if self.use_cuda_graph else 0, _lib.ptr(out),
+                                                    _lib.stream_ptr(dev)))
+        keep.append((z, m32, out))
+        return list(out.split([c["z"].shape[0] for c in calls]))
 
     @torch.no_grad()
     def decode(self, z, codec):
