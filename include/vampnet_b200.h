@@ -61,6 +61,37 @@ typedef struct vnb_weights {
   int32_t rel_sat;
 } vnb_weights;
 
+/* ---- per-request LoRA adapters ------------------------------------------------------------------------------
+ * A fine-tune of the reference is its base model plus rank-8 LoRA on w_qs, w_vs, fc, w_1 and w_2 (transformer.py:22,
+ * 109-114, 70-84); nothing else differs.  Registered adapters are applied per group of batch rows on top of the one
+ * packed base weight set, so one launch serves requests for different fine-tunes.  In every LoRA'd GEMM an adapted
+ * row computes
+ *   acc' = acc + sum_{k<8} u[row, k] * B'[col, k],   u[row, :] = y_bf16[row, :] . A'^T (fp32),
+ * added in fp32 to the tensor-core accumulator before the epilogue's own operations (row scale, rounding, GEGLU,
+ * residual).  Rows of the base (adapter -1) skip the update.  The form is the same for every adapted row wherever it
+ * lands, so batched launches equal the calls made one by one.  It is not bit-identical to a model with the same LoRA
+ * folded into its weights (the fold happens before the bf16 rounding of W).
+ *
+ * vnb_adapter_weights: DEVICE pointers to fp32 tensors owned by the caller and kept alive while the adapter is
+ * registered.  A' = lora_A with the RMSNorm weight folded in (norm_1 for q/v, norm_3 for w_1), stored k-major;
+ * B' = lora_B * alpha / r (alpha = 1, r = 8), rows permuted exactly like the packed weight rows:
+ *   a_qkv (L, d, 16)   [A'_q | A'_v] per input column      b_qkv (L, 2d, 8)  [B'_q rows | B'_v rows] (k has no LoRA)
+ *   a_wo  (L, d, 8)    fc                                  b_wo  (L, d, 8)
+ *   a_w1  (L, d, 8)    w_1 (columns scaled by norm_3)      b_w1  (L, 4d, 8)  rows interleaved like vnb_weights.w1
+ *   a_w2  (L, 2d, 8)   w_2                                 b_w2  (L, d, 8) */
+#define VNB_LORA_RANK 8
+#define VNB_MAX_ADAPTERS 16 /* live adapters per model */
+typedef struct vnb_adapter_weights {
+  const float* a_qkv;
+  const float* b_qkv;
+  const float* a_wo;
+  const float* b_wo;
+  const float* a_w1;
+  const float* b_w1;
+  const float* a_w2;
+  const float* b_w2;
+} vnb_adapter_weights;
+
 /* Mirrors the keyword arguments of VampNet.generate that are live on this path
  * (transformer.py:687-710; SURVEY.md §A.6 lists the dead ones).  The per-step schedule arrays
  * are computed by the host with the reference's own fp32 expressions (mask.py:8-9,
@@ -87,6 +118,14 @@ void vnb_model_destroy(vnb_model* m);
  * codes: (B, C, T) int64 device.  logits: (B, T*Cp, V) fp32 device, i.e. the reference's
  * (B, V, T*Cp) output transposed (the layout generate() permutes to at transformer.py:849). */
 int32_t vnb_forward_codes(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, float* logits, void* stream);
+/* Register an adapter (errors: a NULL pointer, VNB_MAX_ADAPTERS already live); *id in [0, VNB_MAX_ADAPTERS).  Ids of
+ * removed adapters are reused.  Removing an unknown or removed id is an error.  Neither call touches the device. */
+int32_t vnb_adapter_add(vnb_model* m, const vnb_adapter_weights* w, int32_t* id);
+int32_t vnb_adapter_remove(vnb_model* m, int32_t id);
+/* vnb_forward_codes with an adapter per batch row: row_adapter host [B], entries -1 (base) or live ids; NULL = all
+ * base (then this is vnb_forward_codes). */
+int32_t vnb_forward_codes_adapted(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, const int32_t* row_adapter,
+                                  float* logits, void* stream);
 /* VampNet.forward on caller-supplied latents (B, 8C, T) fp32 (transformer.py:617). */
 int32_t vnb_forward_latents(vnb_model* m, const float* latents, int32_t B, int32_t T, float* logits, void* stream);
 /* VampNet.forward(return_activations=True) (transformer.py:617-639, 443-461): as vnb_forward_latents, and the fp32
@@ -124,6 +163,13 @@ typedef struct vnb_gen_group {
 int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
                           const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
                           int64_t* out, void* stream);
+/* vnb_generate_many with an adapter per group: group_adapter host [n_groups], -1 (base) or a live id; NULL = all base
+ * (then this is vnb_generate_many).  Each group equals vnb_generate_many of its rows alone with its adapter, bit for
+ * bit.  A launch with no adapted group runs the plain kernels; otherwise the adapted ones (a second graph per
+ * workspace key; the group -> adapter table is written before every replay and never causes a capture). */
+int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream);
 /* One sampling iteration on caller-supplied logits (B, S, V) fp32 — sample_from_logits +
  * mask_by_random_topk + the where()s around them (transformer.py:849-932).  State is explicit:
  * zflat (B, S) int32 in "t c" order (util.py:39) is updated in place; tokens_out (B, S) int32
@@ -138,14 +184,15 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
  * vnb_launch_count: kernels launched by this library so far in this process (a graph replay adds the
  * number of kernel nodes it contains).
  * vnb_graph_capture_count: generate graphs captured so far (a weight hot swap or a repeated call must not
- * add to it: graphs are cached per (workspace, steps, mask, top_p); the grouping of vnb_generate_many is not part
- * of that key).
+ * add to it: graphs are cached per (workspace, steps, mask, top_p, adapted or not); the grouping of
+ * vnb_generate_many and the group -> adapter table are not part of that key).
  * vnb_profile_begin/end: between the two calls every launch of forward/generate is bracketed by CUDA
  * events on the launching stream (graph replay is bypassed so that the events can be recorded);
  * end() returns the summed device time and launch count per kernel family:
  *   0 embed, 1 rmsnorm, 2 gemm_qkv, 3 attention, 4 gemm_attn_out, 5 gemm_ffn_up, 6 gemm_ffn_down,
- *   7 gemm_classifier, 8 sample+remask, 9 state init/finish. */
-#define VNB_NUM_FAMILIES 10
+ *   7 gemm_classifier, 8 sample+remask, 9 state init/finish, 10 LoRA down-projection (adapted launches only; the
+ *   adapted GEMMs count in their own families). */
+#define VNB_NUM_FAMILIES 11
 uint64_t vnb_launch_count(void);
 uint64_t vnb_graph_capture_count(void);
 
@@ -196,6 +243,15 @@ int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int
 int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
                            void* out2, const float* bias, int32_t T, int32_t Tpad, const float* ss_in,
                            int32_t ss_parts, float inv_d, float eps, void* out_bf16, float* ss_out, void* stream);
+/* Test-only: one adapted GEMM, epi in {QKV, RESID, GEGLU}, with the arguments of vnb_dbg_gemm_fused.  First the
+ * LoRA down-projection u (M, R) fp32 = A . A'^T of every row m with row_adapter[m] >= 0 (R = 16 for QKV, else 8; rows
+ * of the base are not written), then the GEMM whose epilogue adds u[m] . B'[n] to the accumulators of those rows.
+ * adapters[n_adapters] (n_adapters <= VNB_MAX_ADAPTERS) as in vnb_adapter_weights, layer = the layer they are read
+ * at; row_adapter DEVICE [M], entries -1 or < n_adapters. */
+int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                             void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
+                             float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
+                             int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream);
 /* Test-only: the classifier GEMM with the sampling epilogue of the generate loop (VNB_EPI_SAMPLE) alone.
  * N == (C - ncc) * V, V % 128 == 0, V <= 1024; logits x = (A . W^T) * rs + bias with rs as above.
  * zcur (M, C) int32, row m = b*T + t: codebook ncc + cp of row m is sampled iff it holds mask_token.

@@ -14,6 +14,8 @@ LIB_PATH = os.path.join(_HERE, "libvampnet_b200.so")
 EPI_BF16, EPI_QKV, EPI_RESID, EPI_GEGLU, EPI_BIAS_F32 = range(5)
 FAMILIES = ("embed", "rmsnorm", "gemm_qkv", "attention", "gemm_attn_out", "gemm_ffn_up", "gemm_ffn_down",
             "gemm_classifier", "sample_remask", "state")
+LORA_DOWN_FAMILY = 10  # profile family of the LoRA down-projections (adapted launches only); VNB_NUM_FAMILIES = 11
+MAX_ADAPTERS = 16      # VNB_MAX_ADAPTERS
 
 
 class Config(C.Structure):
@@ -28,6 +30,10 @@ class Weights(C.Structure):
         ("norm_f", C.c_void_p), ("wcls", C.c_void_p), ("bcls", C.c_void_p), ("rel_bias", C.c_void_p),
         ("rel_sat", C.c_int32),
     ]
+
+
+class AdapterWeights(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("a_qkv", "b_qkv", "a_wo", "b_wo", "a_w1", "b_w1", "a_w2", "b_w2")]
 
 
 class GenParams(C.Structure):
@@ -60,6 +66,13 @@ _SIGS = {
     "vnb_generate_many": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                       C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p]),
+    "vnb_generate_many_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                              C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32,
+                                              C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_adapter_add": (C.c_int32, [C.c_void_p, C.POINTER(AdapterWeights), C.POINTER(C.c_int32)]),
+    "vnb_adapter_remove": (C.c_int32, [C.c_void_p, C.c_int32]),
+    "vnb_forward_codes_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
+                                              C.c_void_p, C.c_void_p]),
     "vnb_launch_count": (C.c_uint64, []),
     "vnb_graph_capture_count": (C.c_uint64, []),
     "vnb_set_option": (C.c_int32, [C.c_char_p, C.c_int32]),
@@ -86,6 +99,10 @@ _SIGS = {
     "vnb_dbg_gemm_fused": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float,
                                        C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_dbg_gemm_adapted": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float,
+                                         C.c_float, C.c_void_p, C.c_void_p, C.POINTER(AdapterWeights), C.c_int32,
+                                         C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vnb_dbg_gemm_sample": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                         C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,

@@ -139,8 +139,10 @@ struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in w
   bool top_p;  // selects the sampler kernel variant
   int variant;  // GEMM kernel variant baked into the graph (vnb_set_option "gemm_pair")
   bool fused;   // sampler fused into the classifier epilogue (vnb_set_option "fused_sampler")
+  bool adapted;  // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
   bool operator<(const GraphKey& o) const {
-    return std::tie(steps, has_mask, top_p, variant, fused) < std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused);
+    return std::tie(steps, has_mask, top_p, variant, fused, adapted) <
+           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted);
   }
 };
 
@@ -151,6 +153,9 @@ struct Workspace {
   // stride B, rowgrp (B) = the group of every batch row; all three are rewritten before every launch or graph replay
   DevBuf x, y, qk, vT, att, h, logits, zcur, zorig, tokens, conf, n0, dyn, rowgrp, z_in, mask_in, z_out, ssA, ssB, embA,
       partials;
+  // adapted launches: grp_adapter (B) = the adapter of every group (-1: base), rewritten before every launch or replay;
+  // lora_u (M, 16) = the down-projection of the GEMM about to run
+  DevBuf grp_adapter, lora_u;
   int embKp = 0;
   int ss_parts = 0;
   std::vector<GemmPlan> qkv, wo, up, down;
@@ -167,7 +172,7 @@ struct Workspace {
 
 namespace vnb {
 enum { FAM_EMBED = 0, FAM_RMSNORM, FAM_GEMM_QKV, FAM_ATTN, FAM_GEMM_O, FAM_GEMM_UP, FAM_GEMM_DOWN, FAM_GEMM_CLS,
-       FAM_SAMPLE, FAM_STATE, FAM_COUNT };
+       FAM_SAMPLE, FAM_STATE, FAM_LORA_DOWN, FAM_COUNT };
 static unsigned long long g_captures = 0;  // generate graphs captured + instantiated so far
 static unsigned long long g_launches = 0;  // kernels launched by this library (graph replays add their node count)
 void count_launch(unsigned long long n) { g_launches += n; }
@@ -200,6 +205,10 @@ struct vnb_model {
   static constexpr int kMaxSteps = 256;
   static constexpr size_t kMaxWorkspaces = 6;
   unsigned long long use_clock = 0;
+  // registered adapters: host copy of the table and its device image (rewritten before every adapted launch)
+  vnb::AdapterDev adapters[VNB_MAX_ADAPTERS] = {};
+  bool adapter_live[VNB_MAX_ADAPTERS] = {};
+  vnb::DevBuf adapter_tab;
 };
 
 namespace vnb {
@@ -243,6 +252,8 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   CK(ws->n0.alloc(4 * static_cast<size_t>(B), true));
   CK(ws->dyn.alloc(sizeof(SampleDyn) * vnb_model::kMaxSteps * B));
   CK(ws->rowgrp.alloc(sizeof(RowGroup) * B));
+  CK(ws->grp_adapter.alloc(sizeof(int32_t) * B));
+  CK(ws->lora_u.alloc(M * 16 * 4));
   CK(ws->z_in.alloc(M * c.n_codebooks * 8));
   CK(ws->mask_in.alloc(M * c.n_codebooks * 4));
   CK(ws->z_out.alloc(M * c.n_codebooks * 8));
@@ -318,19 +329,40 @@ static int run_embed(vnb_model* m, Workspace* ws, const int32_t* codes_btc, cons
   return 0;
 }
 
+// One LoRA'd GEMM of layer l: plain, or (adapted) the down-projection of its A operand `a` then the adapted epilogue.
+static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int fam, bool adapted, int slot, int l,
+                         const void* a, cudaStream_t st) {
+  if (!adapted) {
+    LAUNCH(fam, launch_gemm(plan, st));
+    return 0;
+  }
+  GemmPlan p = plan;
+  p.lora.table = m->adapter_tab.as<AdapterDev>();
+  p.lora.grp_adapter = ws->grp_adapter.as<int32_t>();
+  p.lora.rowgrp = ws->rowgrp.as<RowGroup>();
+  p.lora.rows_per_grp = ws->T;
+  p.lora.slot = slot;
+  p.lora.layer = l;
+  p.lora.u = ws->lora_u.as<float>();
+  LAUNCH(FAM_LORA_DOWN, launch_lora_down(a, p.M, p.K, p.lora, st));
+  LAUNCH(fam, launch_gemm(p, st));
+  return 0;
+}
+
 // x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.
 static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st, float* acts = nullptr,
-                     const SampleDyn* fused_dyn = nullptr) {
+                     const SampleDyn* fused_dyn = nullptr, bool adapted = false) {
   const vnb_config& c = m->cfg;
   // RMSNorm (transformer.py:43-58) is fused: norm weights are folded into wqkv / w1 / wcls at pack time, the
   // producers of x (embed, attn-out, ffn-down) also emit bf16(x) and per-row sums of squares, and the consumers
   // scale their accumulator rows by rsqrt(mean(x^2) + eps).
   for (int l = 0; l < c.n_layers; ++l) {
-    LAUNCH(FAM_GEMM_QKV, launch_gemm(ws->qkv[l], st));
+    if (run_lora_gemm(m, ws, ws->qkv[l], FAM_GEMM_QKV, adapted, LORA_QKV, l, ws->y.p, st)) return 1;
     LAUNCH(FAM_ATTN, launch_attention(ws->attn, st));
-    LAUNCH(FAM_GEMM_O, launch_gemm(ws->wo[l], st));
-    LAUNCH(FAM_GEMM_UP, launch_gemm(ws->up[l], st));
-    LAUNCH(FAM_GEMM_DOWN, launch_gemm(ws->down[l], st));
+    if (run_lora_gemm(m, ws, ws->wo[l], FAM_GEMM_O, adapted, LORA_WO, l, ws->att.p, st) ||
+        run_lora_gemm(m, ws, ws->up[l], FAM_GEMM_UP, adapted, LORA_W1, l, ws->y.p, st) ||
+        run_lora_gemm(m, ws, ws->down[l], FAM_GEMM_DOWN, adapted, LORA_W2, l, ws->h.p, st))
+      return 1;
     if (acts)  // return_activations: the residual stream after this layer (transformer.py:455-456)
       CK(cudaMemcpyAsync(acts + static_cast<size_t>(l) * ws->M * c.d_model, ws->x.p, ws->x.n, cudaMemcpyDeviceToDevice, st));
   }
@@ -391,6 +423,27 @@ static int one_group_rows(int rows, const RowGroup** out) {
   return 0;
 }
 
+// Adapter ids of a launch (host, n entries; NULL = none): each -1 or a live id.
+static int check_adapter_ids(const vnb_model* m, const int32_t* ids, int n, const char* who) {
+  if (!ids) return 0;
+  for (int i = 0; i < n; ++i)
+    if (ids[i] != -1 && (ids[i] < 0 || ids[i] >= VNB_MAX_ADAPTERS || !m->adapter_live[ids[i]]))
+      return fail("%s: entry %d names adapter %d, which is not registered", who, i, ids[i]);
+  return 0;
+}
+static bool any_adapted(const int32_t* ids, int n) {
+  for (int i = 0; ids && i < n; ++i)
+    if (ids[i] >= 0) return true;
+  return false;
+}
+// Stream-ordered writes of the adapter table and the group -> adapter map of an adapted launch (pageable sources:
+// staged before the calls return).
+static int stage_adapters(vnb_model* m, Workspace* ws, const int32_t* grp_adapter, int n_groups, cudaStream_t st) {
+  CK(cudaMemcpyAsync(m->adapter_tab.p, m->adapters, sizeof(m->adapters), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(ws->grp_adapter.p, grp_adapter, sizeof(int32_t) * n_groups, cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
 }  // namespace vnb
 
 using namespace vnb;
@@ -419,23 +472,67 @@ int32_t vnb_model_create(const vnb_config* cfg, const vnb_weights* w, vnb_model*
   auto* m = new vnb_model();
   m->cfg = *cfg;
   m->w = *w;
+  if (m->adapter_tab.alloc(sizeof(m->adapters), true) != cudaSuccess) {
+    delete m;
+    return fail("vnb_model_create: cannot allocate the adapter table");
+  }
   *out = m;
+  return 0;
+}
+
+int32_t vnb_adapter_add(vnb_model* m, const vnb_adapter_weights* w, int32_t* id) {
+  if (!m || !w || !id) return fail("vnb_adapter_add: null argument");
+  const float* ptrs[2 * LORA_SLOTS] = {w->a_qkv, w->b_qkv, w->a_wo, w->b_wo, w->a_w1, w->b_w1, w->a_w2, w->b_w2};
+  static const char* names[2 * LORA_SLOTS] = {"a_qkv", "b_qkv", "a_wo", "b_wo", "a_w1", "b_w1", "a_w2", "b_w2"};
+  for (int i = 0; i < 2 * LORA_SLOTS; ++i)
+    if (!ptrs[i]) return fail("vnb_adapter_add: %s is NULL", names[i]);
+  int slot = -1;
+  for (int i = 0; i < VNB_MAX_ADAPTERS && slot < 0; ++i)
+    if (!m->adapter_live[i]) slot = i;
+  if (slot < 0) return fail("vnb_adapter_add: the adapter table is full (%d live adapters)", VNB_MAX_ADAPTERS);
+  AdapterDev& a = m->adapters[slot];
+  for (int s = 0; s < LORA_SLOTS; ++s) { a.a[s] = ptrs[2 * s]; a.b[s] = ptrs[2 * s + 1]; }
+  m->adapter_live[slot] = true;
+  *id = slot;
+  return 0;
+}
+
+int32_t vnb_adapter_remove(vnb_model* m, int32_t id) {
+  if (!m) return fail("vnb_adapter_remove: null model");
+  if (id < 0 || id >= VNB_MAX_ADAPTERS || !m->adapter_live[id])
+    return fail("vnb_adapter_remove: adapter %d is not registered", id);
+  m->adapter_live[id] = false;
+  m->adapters[id] = AdapterDev{};
   return 0;
 }
 
 void vnb_model_destroy(vnb_model* m) { delete m; }
 
-int32_t vnb_forward_codes(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, float* logits, void* stream) {
+int32_t vnb_forward_codes_adapted(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, const int32_t* row_adapter,
+                                  float* logits, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (B < 1 || T < 1) return fail("vnb_forward_codes: need B >= 1 and T >= 1 (got %d, %d)", B, T);
+  if (check_adapter_ids(m, row_adapter, B, "vnb_forward_codes_adapted")) return 1;
+  const bool adapted = any_adapted(row_adapter, B);
   Workspace* ws;
   if (get_workspace(m, B, T, &ws)) return 1;
+  if (adapted) {  // batch row b is its own group
+    std::vector<RowGroup> rowgrp(B);
+    for (int b = 0; b < B; ++b) rowgrp[b] = RowGroup{b, b};
+    CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+    if (stage_adapters(m, ws, row_adapter, B, st)) return 1;
+  }
   const vnb_config& c = m->cfg;
   // (B,C,T) int64 -> (B,T,C) int32, no masking (mask = zeros)
   LAUNCH(FAM_STATE, launch_gen_init(codes, nullptr, ws->zcur.as<int32_t>(), ws->zorig.as<int32_t>(), ws->n0.as<int32_t>(),
                                     nullptr, 1, B, c.n_codebooks, T, /*ncc=*/c.n_codebooks, c.vocab_size, st));
   if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
   m->last = ws;
-  return run_stack(m, ws, logits, st);
+  return run_stack(m, ws, logits, st, nullptr, nullptr, adapted);
+}
+
+int32_t vnb_forward_codes(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, float* logits, void* stream) {
+  return vnb_forward_codes_adapted(m, codes, B, T, nullptr, logits, stream);
 }
 
 int32_t vnb_forward_latents(vnb_model* m, const float* latents, int32_t B, int32_t T, float* logits, void* stream) {
@@ -475,7 +572,7 @@ static int fused_sampler_enabled() {
 }
 
 static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int steps, int64_t* out,
-                            cudaStream_t st, bool use_top_p, bool fused) {
+                            cudaStream_t st, bool use_top_p, bool fused, bool adapted) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
   // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
@@ -494,10 +591,10 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
     if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
     const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
     if (fused) {
-      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i)) return 1;
+      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
     } else {
-      if (run_stack(m, ws, ws->logits.as<float>(), st)) return 1;
+      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_step_dev(sa, dyn_i, st, use_top_p));
     }
     ++g_launches;  // sample step = two kernels
@@ -507,9 +604,9 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   return 0;
 }
 
-int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
-                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
-                          int64_t* out, void* stream) {
+int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
   if (!gamma || !groups) return fail("vnb_generate_many: gamma and groups are required");
@@ -527,6 +624,8 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
     total += q.rows;
   }
   if (total != B) return fail("vnb_generate_many: group rows sum to %lld, not B = %d", total, B);
+  if (check_adapter_ids(m, group_adapter, n_groups, "vnb_generate_many_adapted")) return 1;
+  const bool adapted = any_adapted(group_adapter, n_groups);
   Workspace* ws;
   if (get_workspace(m, B, T, &ws)) return 1;
   m->last = ws;
@@ -553,10 +652,11 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
   }
   CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * dyn.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+  if (adapted && stage_adapters(m, ws, group_adapter, n_groups, st)) return 1;
   const bool fused = fused_sampler_enabled() != 0 && !use_top_p && ws->can_fuse;
   if (!fused && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
-  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused);
+  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted);
 
   const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
   CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
@@ -564,7 +664,7 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
   const int64_t* gz = ws->z_in.as<int64_t>();
   const int32_t* gmask = mask ? ws->mask_in.as<int32_t>() : nullptr;
   int64_t* gout = ws->z_out.as<int64_t>();
-  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused};
+  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted};
   auto it = ws->graphs.find(key);
   if (it == ws->graphs.end()) {
     cudaStream_t cap;
@@ -573,7 +673,7 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cap); return fail("begin capture: %s", cudaGetErrorString(e)); }
     const unsigned long long before = g_launches;
-    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused);
+    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted);
     const unsigned long long in_graph = g_launches - before;
     g_launches = before;
     e = cudaStreamEndCapture(cap, &graph);
@@ -597,6 +697,12 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
   g_launches += ws->graph_kernels[key];
   CK(cudaMemcpyAsync(out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
+                          int64_t* out, void* stream) {
+  return vnb_generate_many_adapted(m, z, mask, B, T, steps, gamma, groups, n_groups, nullptr, use_graph, out, stream);
 }
 
 // One call is the one-group launch.
@@ -721,6 +827,51 @@ int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M,
   p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
   if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                             void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
+                             float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
+                             int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
+  if (epi != VNB_EPI_QKV && epi != VNB_EPI_RESID && epi != VNB_EPI_GEGLU)
+    return fail("vnb_dbg_gemm_adapted: epilogue %d has no adapted variant", epi);
+  if (!adapters || n_adapters < 1 || n_adapters > VNB_MAX_ADAPTERS || !row_adapter || !u || layer < 0)
+    return fail("vnb_dbg_gemm_adapted: need 1..%d adapters, a row map, u and layer >= 0", VNB_MAX_ADAPTERS);
+  if ((out_bf16 != nullptr || ss_out != nullptr) && epi != VNB_EPI_RESID)
+    return fail("vnb_dbg_gemm_adapted: out_bf16 / ss_out need the RESID epilogue");
+  if ((out_bf16 == nullptr) != (ss_out == nullptr)) return fail("vnb_dbg_gemm_adapted: out_bf16 and ss_out go together");
+  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_adapted: ss_parts must be >= 1");
+  if (epi == VNB_EPI_QKV && (out2 == nullptr || N % 96 != 0 || T < 1 || Tpad < T))
+    return fail("vnb_dbg_gemm_adapted: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  std::vector<AdapterDev> tab(VNB_MAX_ADAPTERS);
+  for (int i = 0; i < n_adapters; ++i) {
+    const vnb_adapter_weights& w = adapters[i];
+    const float* ptrs[2 * LORA_SLOTS] = {w.a_qkv, w.b_qkv, w.a_wo, w.b_wo, w.a_w1, w.b_w1, w.a_w2, w.b_w2};
+    for (int s = 0; s < LORA_SLOTS; ++s) { tab[i].a[s] = ptrs[2 * s]; tab[i].b[s] = ptrs[2 * s + 1]; }
+  }
+  std::vector<RowGroup> rowgrp(M);
+  for (int i = 0; i < M; ++i) rowgrp[i] = RowGroup{i, i};  // row m is its own group: grp_adapter = row_adapter
+  GemmPlan p;
+  const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
+  if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, nullptr, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
+  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
+  if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
+  DevBuf tab_dev, grp_dev;
+  CK(tab_dev.alloc(sizeof(AdapterDev) * VNB_MAX_ADAPTERS));
+  CK(grp_dev.alloc(sizeof(RowGroup) * M));
+  CK(cudaMemcpyAsync(tab_dev.p, tab.data(), sizeof(AdapterDev) * VNB_MAX_ADAPTERS, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * M, cudaMemcpyHostToDevice, st));
+  p.lora.table = tab_dev.as<AdapterDev>();
+  p.lora.grp_adapter = row_adapter;
+  p.lora.rowgrp = grp_dev.as<RowGroup>();
+  p.lora.rows_per_grp = 1;
+  p.lora.slot = epi == VNB_EPI_QKV ? LORA_QKV : epi == VNB_EPI_GEGLU ? LORA_W1 : (K == N ? LORA_WO : LORA_W2);
+  p.lora.layer = layer;
+  p.lora.u = u;
+  CK(launch_lora_down(A, M, K, p.lora, st));
+  CK(launch_gemm(p, st));
+  CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
   return 0;
 }
 int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,

@@ -38,6 +38,7 @@ constexpr int SBIAS_BYTES = BN * 4;                // EPI_SAMPLE: the tile's bia
 constexpr int RING_BYTES = STAGES * STAGE_BYTES;  // 192 KiB
 constexpr int ACC_PITCH = BN + 1;                 // fp32 accumulator tile: odd pitch, every epilogue read is conflict-free
 static_assert(BM * ACC_PITCH * 4 <= RING_BYTES, "the accumulator tile overlays the ring");
+static_assert(BM * ACC_PITCH * 4 + 4 * BM + 16 + 32 * BM <= RING_BYTES, "the adapted epilogue's row table follows it");
 constexpr int GEMM_SMEM = RING_BYTES + SBIAS_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 static_assert(GEMM_SMEM <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
 constexpr int GEMM_THREADS = 256 + 32;            // two consumer warpgroups + the producer warp
@@ -67,6 +68,8 @@ struct GemmArgs {
   const RowGroup* rowgrp;   // (B) group of every batch row
   float4* partials;
   int C, ncc, V, mask_token;
+  // ---- adapted variants (ADAPT): per-row LoRA update of the accumulators, see lora_update() ----
+  AdapterRefs lora;
 };
 
 __device__ __forceinline__ float gelu_tanh(float x) {
@@ -176,13 +179,80 @@ __device__ __forceinline__ void acc_ld_x32(uint32_t addr, uint32_t (&v)[32]) {
   for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(lds_f32(addr + 4u * j));
 }
 
+// LoRA update of the accumulator tile (adapted variants only; DESIGN.md §1): for every adapted row m of the tile and
+// every column n, acc[m][n] += sum_k u[m][k] * B'[n][k], k = 0..7 in a fixed fma chain, added before anything the
+// epilogue does (row scale, rounding, GEGLU, residual).  Base rows (adapter -1) are skipped, not updated by zero.  The
+// arithmetic of a row depends only on its own u and its adapter's B', never on which rows share its tile.
+// The adapter and the u of every tile row are staged once in `scratch` (free shared memory past the accumulator tile).
+// Then, per adapter present in the tile, thread t keeps B' of its four columns (t % 64) + 64 j in registers and updates
+// them in the rows (t / 64) + 4 i of that adapter: a warp covers 32 consecutive columns of one row (conflict-free), and
+// the row's u is a broadcast shared-memory read.
+template <int EPI>
+__device__ __forceinline__ void lora_update(const GemmArgs& g, uint8_t* scratch, uint32_t acc_tile, int m0, int n0) {
+  int uoff = 0, brow0 = n0;
+  if constexpr (EPI == VNB_EPI_QKV) {
+    // columns [0, d) q, [d, 2d) k (w_ks has no LoRA: no update), [2d, 3d) v; a 256-column tile lies in one of them
+    const int d = g.N / 3;
+    if (n0 >= d && n0 < 2 * d) return;
+    if (n0 >= 2 * d) { uoff = 8; brow0 = n0 - d; }
+  }
+  const AdapterRefs& L = g.lora;
+  const int t = static_cast<int>(threadIdx.x);
+  int32_t* sid = reinterpret_cast<int32_t*>(scratch);               // adapter of tile row r (-1: base, or past M)
+  uint32_t* smask = reinterpret_cast<uint32_t*>(scratch + 4 * BM);  // adapters present among the rows of warps 0..3
+  float4* su = reinterpret_cast<float4*>(scratch + 4 * BM + 16);     // u of tile row r: su[2 r], su[2 r + 1]
+  constexpr int R = EPI == VNB_EPI_QKV ? 16 : 8;
+  if (t < BM) {
+    const int m = m0 + t;
+    const int id = m < g.M ? L.grp_adapter[L.rowgrp[m / L.rows_per_grp].group] : -1;
+    sid[t] = id;
+    if (id >= 0) {
+      su[2 * t] = __ldg(reinterpret_cast<const float4*>(L.u + static_cast<size_t>(m) * R + uoff));
+      su[2 * t + 1] = __ldg(reinterpret_cast<const float4*>(L.u + static_cast<size_t>(m) * R + uoff + 4));
+    }
+    uint32_t bits = 0;
+    for (int a = 0; a < VNB_MAX_ADAPTERS; ++a) bits |= __ballot_sync(0xffffffffu, id == a) ? (1u << a) : 0u;
+    if ((t & 31) == 0) smask[t >> 5] = bits;
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  const uint32_t present = smask[0] | smask[1] | smask[2] | smask[3];
+  const int nb = EPI == VNB_EPI_QKV ? 2 * (g.N / 3) : g.N;  // rows of B' per layer
+  const int c0 = t & 63, rq = t >> 6;
+  for (int a = 0; a < VNB_MAX_ADAPTERS; ++a) {
+    if (!((present >> a) & 1u)) continue;
+    const float* bp = L.table[a].b[L.slot] + (static_cast<size_t>(L.layer) * nb + brow0 + c0) * 8;
+    float4 b0[4], b1[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      b0[j] = __ldg(reinterpret_cast<const float4*>(bp + 64 * 8 * j));
+      b1[j] = __ldg(reinterpret_cast<const float4*>(bp + 64 * 8 * j + 4));
+    }
+#pragma unroll 4
+    for (int i = 0; i < BM / 4; ++i) {
+      const int r = rq + 4 * i;
+      if (sid[r] != a) continue;
+      const float4 ua = su[2 * r], ub = su[2 * r + 1];
+      const uint32_t row_addr = acc_tile + 4u * (r * ACC_PITCH + c0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float s = __fmul_rn(ua.x, b0[j].x);
+        s = __fmaf_rn(ua.y, b0[j].y, s); s = __fmaf_rn(ua.z, b0[j].z, s); s = __fmaf_rn(ua.w, b0[j].w, s);
+        s = __fmaf_rn(ub.x, b1[j].x, s); s = __fmaf_rn(ub.y, b1[j].y, s); s = __fmaf_rn(ub.z, b1[j].z, s);
+        s = __fmaf_rn(ub.w, b1[j].w, s);
+        const uint32_t addr = row_addr + 4u * (64 * j);
+        sts_f32(addr, __fadd_rn(lds_f32(addr), s));
+      }
+    }
+  }
+}
+
 // PAIR = true: clusters of two CTAs on vertically adjacent 128 x 256 tiles (the same 256 W rows).  Each CTA fetches
 // half of the W tile (128 rows) and the TMA multicasts it into both CTAs' shared memory, so per CTA the W bytes pulled
 // from L2 are halved; a stage is refilled only when the consumer warps of both CTAs have released it.  Every output
 // element sees the same operands in the same K order as in the single-CTA variant: the two are bit-identical.  On an
 // H100 the single-CTA kernel is faster (the pair couples the two CTAs' progress and constrains their placement; same-
 // box A/B at the default bench workload: 403 vs 333 TFLOP/s for the GEMM family), so it is the default.
-template <int EPI, bool PAIR>
+template <int EPI, bool PAIR, bool ADAPT = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmArgs g) {
@@ -286,6 +356,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         sts_f32(p0 + 4u * (8 * ACC_PITCH) + 32u * i + 4, acc[4 * i + 3]);
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
+      if constexpr (ADAPT) {
+        lora_update<EPI>(g, smem + BM * ACC_PITCH * 4, acc_tile, m0, n0);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
     }
     // ===================== epilogue =====================
     constexpr bool kWide = gemm_epi_warps<EPI>() == 8;
@@ -504,6 +578,12 @@ static cudaError_t init_epi() {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
   if (e != cudaSuccess) return e;
+  if constexpr (EPI == VNB_EPI_QKV || EPI == VNB_EPI_RESID || EPI == VNB_EPI_GEGLU) {
+    e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
+    if (e != cudaSuccess) return e;
+  }
   cudaLaunchConfig_t q = {};
   q.gridDim = dim3(2 * device_sm_count());
   q.blockDim = dim3(GEMM_THREADS);
@@ -537,7 +617,7 @@ int get_gemm_max_clusters() {
 }
 
 // One CTA per output tile (the accumulator tile overlays the operand ring, so a CTA does not start a second tile).
-template <int EPI>
+template <int EPI, bool ADAPT = false>
 static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t st) {
   cudaError_t e = init_epi<EPI>();
   if (e != cudaSuccess) return e;
@@ -552,10 +632,10 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true>, p.tmA, p.tmBh, g);
+    return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true, ADAPT>, p.tmA, p.tmBh, g);
   }
   const int tiles = ((g.M + BM - 1) / BM) * (g.N / BN);
-  gemm_wgmma_kernel<EPI, false><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
+  gemm_wgmma_kernel<EPI, false, ADAPT><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
   return cudaGetLastError();
 }
 
@@ -567,6 +647,16 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
   g.ss_parts = p.ss_parts; g.inv_d = p.inv_d; g.eps = p.eps;
   g.zcur = p.zcur; g.dyn = p.dyn; g.rowgrp = p.rowgrp; g.partials = reinterpret_cast<float4*>(p.partials);
   g.C = p.C; g.ncc = p.ncc; g.V = p.V; g.mask_token = p.mask_token;
+  g.lora = p.lora;
+  if (p.lora.table != nullptr) {
+    if (!p.lora.grp_adapter || !p.lora.rowgrp || !p.lora.u || p.lora.rows_per_grp < 1) return cudaErrorInvalidValue;
+    switch (p.epi) {
+      case VNB_EPI_QKV: return launch_epi<VNB_EPI_QKV, true>(p, g, st);
+      case VNB_EPI_RESID: return launch_epi<VNB_EPI_RESID, true>(p, g, st);
+      case VNB_EPI_GEGLU: return launch_epi<VNB_EPI_GEGLU, true>(p, g, st);
+      default: return cudaErrorInvalidValue;  // the embedding and the classifier carry no LoRA
+    }
+  }
   switch (p.epi) {
     case VNB_EPI_BF16: return launch_epi<VNB_EPI_BF16>(p, g, st);
     case VNB_EPI_QKV: return launch_epi<VNB_EPI_QKV>(p, g, st);

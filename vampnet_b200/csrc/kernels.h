@@ -50,6 +50,26 @@ struct RowGroup {
   int32_t group, first;
 };
 
+// ---- per-request LoRA adapters (DESIGN.md §1) ----
+// One registered adapter: the device pointers of vnb_adapter_weights, indexed by LoRA slot (a[s], b[s]).
+enum { LORA_QKV = 0, LORA_WO, LORA_W1, LORA_W2, LORA_SLOTS };
+struct AdapterDev {
+  const float* a[LORA_SLOTS];  // A' (L, K, R_s) fp32, k-major
+  const float* b[LORA_SLOTS];  // B' (L, N_s, 8) fp32
+};
+// How the rows of a launch find their adapter: row m -> batch row m / rows_per_grp -> rowgrp[.].group ->
+// grp_adapter[group] (-1: base row, no update) -> table[id].
+struct AdapterRefs {
+  const AdapterDev* table = nullptr;
+  const int32_t* grp_adapter = nullptr;
+  const RowGroup* rowgrp = nullptr;
+  int rows_per_grp = 1;
+  int slot = 0, layer = 0;
+  float* u = nullptr;  // (M, R) the down-projection of every adapted row, R = 16 for LORA_QKV ([q | v]), else 8
+};
+// u = y . A'^T for every adapted row of y (M, K) bf16; base rows are not touched
+cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, cudaStream_t st);
+
 // ---- GEMM ----
 struct GemmPlan {
   CUtensorMap tmA, tmB;
@@ -71,6 +91,8 @@ struct GemmPlan {
   const RowGroup* rowgrp = nullptr;  // (B) group of every batch row
   void* partials = nullptr;          // (M * Cp * V/128) float4 records, see sample_combine_kernel
   int C = 0, ncc = 0, V = 0, mask_token = 0;
+  // adapted variant of QKV / RESID / GEGLU (null table: the plain kernel): acc += u[row] . B'[col] for adapted rows
+  AdapterRefs lora;
 };
 // Fills the tensor maps; A (M,K) bf16, W (N,K) bf16.
 bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out, void* out2,

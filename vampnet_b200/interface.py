@@ -135,6 +135,16 @@ class Interface(torch.nn.Module):
         where = () if name == "default" else ("loras", name)
         self.reload(coarse_ckpt=self._cached(*where, "coarse.pth"), c2f_ckpt=self._cached(*where, "c2f.pth"))
 
+    def add_finetuned(self, name: str):
+        """Register the fine-tune `name` (loras/<name>/{coarse,c2f}.pth, resolved as load_finetuned resolves them) as a
+        per-request adapter of the live coarse and c2f models: vamp / vamp_many requests then take adapter=name, and
+        requests for different fine-tunes share launches.  The live models stay as they are (see load_finetuned for
+        swapping a fine-tune in)."""
+        coarse, c2f = self._cached("loras", name, "coarse.pth"), self._cached("loras", name, "c2f.pth")
+        self.coarse.add_adapter(name, coarse)
+        if self.c2f is not None:
+            self.c2f.add_adapter(name, c2f)
+
     def reload(self, coarse_ckpt: str = None, c2f_ckpt: str = None):
         """Swap checkpoints (interface.py:146-174); a checkpoint already loaded is skipped.  A checkpoint of the same
         architecture is hot-swapped into the live model (VampNet.swap_checkpoint: packed device buffers rewritten in
@@ -322,17 +332,19 @@ class Interface(torch.nn.Module):
     _C2F_KWARGS = dict(typical_filtering=True, _sampling_steps=2)
 
     def vamp(self, codes: torch.Tensor, mask: torch.Tensor, batch_size: int = 1, feedback_steps: int = 1,
-             time_stretch_factor: int = 1, return_mask: bool = False, **kwargs):
+             time_stretch_factor: int = 1, return_mask: bool = False, adapter: str = None, **kwargs):
         """codes, mask (1|B, 14, T) -> (B, 14, T'): coarse stage (`feedback_steps` passes, kwargs forwarded to
         generate) then the fine stage, which the reference pins to 2 sampling steps with default temperature
-        (interface.py:545-551).  time_stretch_factor k > 1 inserts k-1 always-masked frames after every frame."""
+        (interface.py:545-551).  time_stretch_factor k > 1 inserts k-1 always-masked frames after every frame.
+        adapter: a fine-tune registered with add_finetuned, applied in both stages (None: the live models)."""
         z, mask = self._vamp_inputs(codes, mask, batch_size, time_stretch_factor)
+        with_adapter = {} if adapter is None else dict(adapter=adapter)
         zv = z
         for i in range(feedback_steps):
-            zv, coarse_start = self.coarse_vamp(zv, mask=mask, return_mask=True, **kwargs)
+            zv, coarse_start = self.coarse_vamp(zv, mask=mask, return_mask=True, **with_adapter, **kwargs)
             coarse_start = coarse_start.roll(shifts=(i + 1) % feedback_steps, dims=-1)
         zv, fine_start = self.coarse_to_fine(self._with_fine_books(z, zv), mask=mask, return_mask=True,
-                                             **self._C2F_KWARGS)
+                                             **self._C2F_KWARGS, **with_adapter)
         return self._vamp_result(z, zv, coarse_start, fine_start, return_mask)
 
     @torch.inference_mode()
@@ -355,7 +367,9 @@ class Interface(torch.nn.Module):
             q["z"], q["mask"] = self._vamp_inputs(q["codes"], q["mask"], q["batch_size"], q["time_stretch_factor"])
             q["zv"] = q["z"]
             seed, key = r.pop("seed", None), r.pop("philox_key", None)
-            q["gen"] = r
+            adapter = r.pop("adapter", None)
+            q["with_adapter"] = {} if adapter is None else dict(adapter=adapter)
+            q["gen"] = dict(r, **q["with_adapter"])
 
             def keys(n, seed=seed, key=key):
                 return [key if key is not None else draw_philox_key(seed) for _ in range(n)]
@@ -375,7 +389,7 @@ class Interface(torch.nn.Module):
                 q["zv"], start = self._coarse_stitch(q["zv"], plan, [next(results) for _ in plan], True)
                 q["coarse_start"] = start.roll(shifts=(i + 1) % q["feedback_steps"], dims=-1)
         plans = [self._c2f_plan(self._with_fine_books(q["z"], q["zv"]), q["mask"]) for q in reqs]
-        calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **self._C2F_KWARGS)
+        calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **self._C2F_KWARGS, **q["with_adapter"])
                  for q, (chunks, _) in zip(reqs, plans) for c, k in zip(chunks, q["c2f_keys"])]
         results = iter(self.c2f.generate_many(self.codec, calls))
         out = []

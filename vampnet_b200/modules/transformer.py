@@ -183,6 +183,36 @@ def draw_philox_key(seed=None) -> int:
     return int(torch.randint(0, 2 ** 62, (1,)).item())
 
 
+# the five LoRA'd projections of every layer (reference transformer.py:109-114, 70-84): what a fine-tune differs in
+LORA_MODULES = ("self_attn.w_qs", "self_attn.w_vs", "self_attn.fc", "feed_forward.w_1", "feed_forward.w_2")
+
+
+def pack_adapter(lora: dict, norm1: torch.Tensor, norm3: torch.Tensor, d: int, device) -> dict:
+    """A' / B' of one adapter in the layout include/vampnet_b200.h: vnb_adapter_weights documents.
+    lora[(layer, module)] = (lora_A (8, in), lora_B (out, 8)); norm1 / norm3 (L, d) the base model's RMSNorm weights.
+    A' = lora_A with the norm folded into its columns (as wqkv / w1 get it), k-major; B' = lora_B * alpha / r with rows
+    permuted like the packed weight rows (w1: 128 value rows then 128 gate rows per 256-row tile).  All fp32."""
+    L = norm1.shape[0]
+    s = LORA_ALPHA / LORA_R
+    f = lambda t: t.to(device, torch.float32)
+    out = {k: [] for k in ("a_qkv", "b_qkv", "a_wo", "b_wo", "a_w1", "b_w1", "a_w2", "b_w2")}
+    nt = (2 * d) // 128
+    for l in range(L):
+        (aq, bq), (av, bv), (ao, bo), (a1, b1), (a2, b2) = [tuple(map(f, lora[(l, m)])) for m in LORA_MODULES]
+        n1, n3 = f(norm1[l]), f(norm3[l])
+        out["a_qkv"].append(torch.cat([(aq * n1[None, :]).t(), (av * n1[None, :]).t()], 1))   # (d, 16)
+        out["b_qkv"].append(torch.cat([bq, bv], 0) * s)                                      # (2d, 8)
+        out["a_wo"].append(ao.t())
+        out["b_wo"].append(bo * s)
+        out["a_w1"].append((a1 * n3[None, :]).t())
+        b1s = b1 * s                                                                         # (4d, 8): [value 2d | gate 2d]
+        out["b_w1"].append(torch.cat([b1s[:2 * d].view(nt, 128, LORA_R), b1s[2 * d:].view(nt, 128, LORA_R)], 1)
+                           .reshape(4 * d, LORA_R))
+        out["a_w2"].append(a2.t())
+        out["b_w2"].append(b2 * s)
+    return {k: torch.stack(v).contiguous() for k, v in out.items()}
+
+
 # generate_many() splits a launch whose B*T would exceed this many rows: M = 24576 is the largest GEMM height the
 # benchmarks measure (BASELINE.json configs[4], B = 8 at T = 3072)
 MANY_MAX_ROWS = 24576
@@ -237,6 +267,8 @@ class VampNet(nn.Module):
         self._packed = None       # dict of device tensors kept alive for the handle
         self._packed_key = None
         self._packed_codec = None
+        self._adapters = {}       # name -> packed A' / B' (pack_adapter), registered with every handle
+        self._adapter_ids = {}    # name -> id in the live handle's adapter table
         self.use_cuda_graph = True
         self.eval()
 
@@ -249,6 +281,7 @@ class VampNet(nn.Module):
         if getattr(self, "_handle", None) is not None:
             _lib.lib().vnb_model_destroy(self._handle)
         self._handle = None
+        self._adapter_ids = {}
         self._packed = None
         self._packed_key = None
         self._packed_codec = None
@@ -268,12 +301,121 @@ class VampNet(nn.Module):
                 "position bias and different projection names; this implementation covers the flash_attn=False "
                 "architecture the released VampNet checkpoints use (conf/vampnet.yml:33)")
         live = self._handle is not None and getattr(self, "_packed_codec", None) is not None
+        # registered adapters belong to the current base: a new base (or a folded fine-tune) drops them
+        drop = bool(getattr(self, "_adapters", None)) and self._differing_base_tensor(state_dict) is not None
         if not live:
             self._invalidate()
-            return super().load_state_dict(state_dict, *a, **k)
-        result = super().load_state_dict(state_dict, *a, **k)
-        self.repack()
+            result = super().load_state_dict(state_dict, *a, **k)
+        else:
+            result = super().load_state_dict(state_dict, *a, **k)
+            self.repack()
+        if drop or (getattr(self, "_adapters", None) and self._is_folded()):
+            self._drop_adapters()
         return result
+
+    # ------------------------------------------------------------------ per-request adapters
+    def _differing_base_tensor(self, state_dict):
+        """Name of the first non-LoRA tensor of state_dict that differs from this model's (shape or value), or None."""
+        params = dict(self.named_parameters())
+        for name, t in state_dict.items():
+            if ".lora_" in name or name not in params:
+                continue
+            p = params[name]
+            if tuple(t.shape) != tuple(p.shape) or not torch.equal(t.detach().to(p.device, p.dtype), p.detach()):
+                return name
+        return None
+
+    def _is_folded(self) -> bool:
+        return any(bool((p != 0).any()) for n, p in self.named_parameters() if n.endswith("lora_B"))
+
+    def _drop_adapters(self):
+        lib = _lib.lib() if self._handle is not None else None
+        for name, i in self._adapter_ids.items():
+            _lib.check(lib.vnb_adapter_remove(self._handle, i))
+        self._adapters, self._adapter_ids = {}, {}
+
+    @torch.no_grad()
+    def add_adapter(self, name: str, location_or_state_dict):
+        """Register a fine-tune of this base model as a per-request adapter: generate(adapter=name) and
+        forward_codes(adapter=name) then apply its LoRA (rank 8 on w_qs, w_vs, fc, w_1, w_2) to their rows only, on top
+        of the shared base weights.  Takes a checkpoint in the layout load_finetuned reads (a path or a loaded dict with
+        'state_dict' and 'metadata'), or a plain state dict.  Refuses another architecture, a checkpoint whose non-LoRA
+        tensors differ from this model's, a rank other than 8, and a live model that is itself a folded fine-tune."""
+        blob = location_or_state_dict
+        if not isinstance(blob, dict):
+            blob = torch.load(str(blob), map_location="cpu", weights_only=False)
+        sd = blob.get("state_dict", blob) if isinstance(blob.get("state_dict", None), dict) else blob
+        if "metadata" in blob:
+            import inspect
+            defaults = {k: v.default for k, v in inspect.signature(type(self).__init__).parameters.items()}
+            want = dict(blob["metadata"].get("kwargs", {}))
+            bad = [k for k, v in self.architecture().items() if want.get(k, defaults[k]) != v]
+            if bad:
+                raise ValueError(f"add_adapter({name!r}): the checkpoint's architecture differs ({bad[0]} = "
+                                 f"{want.get(bad[0], defaults[bad[0]])}, this model has {self.architecture()[bad[0]]})")
+        if self._is_folded():
+            raise ValueError(f"add_adapter({name!r}): the live model carries a non-zero lora_B (a folded fine-tune); "
+                             "adapters apply on top of a base model only")
+        lora = {}
+        for l in range(self.n_layers):
+            for m in LORA_MODULES:
+                key = f"transformer.layers.{l}.{m}"
+                if key + ".lora_A" not in sd or key + ".lora_B" not in sd:
+                    raise ValueError(f"add_adapter({name!r}): {key}.lora_A / lora_B missing: not a LoRA fine-tune of "
+                                     "this architecture")
+                a, b = sd[key + ".lora_A"], sd[key + ".lora_B"]
+                prm = self.get_submodule(key).weight
+                if a.shape[0] != LORA_R or b.shape[1] != LORA_R:
+                    raise ValueError(f"add_adapter({name!r}): {key} has LoRA rank {a.shape[0]}; only rank {LORA_R} "
+                                     "is supported")
+                if tuple(a.shape) != (LORA_R, prm.shape[1]) or tuple(b.shape) != (prm.shape[0], LORA_R):
+                    raise ValueError(f"add_adapter({name!r}): {key} LoRA shapes {tuple(a.shape)}, {tuple(b.shape)} do "
+                                     "not fit this architecture")
+                lora[(l, m)] = (a, b)
+        diff = self._differing_base_tensor(sd)
+        if diff is not None:
+            raise ValueError(f"add_adapter({name!r}): {diff} differs from the live model's: the checkpoint is not a "
+                             "fine-tune of this base")
+        if name in self._adapters:
+            self.remove_adapter(name)
+        if len(self._adapters) >= _lib.MAX_ADAPTERS:
+            raise ValueError(f"add_adapter({name!r}): {_lib.MAX_ADAPTERS} adapters are already registered")
+        lay = self.transformer.layers
+        norm1 = torch.stack([x.norm_1.weight.detach() for x in lay])
+        norm3 = torch.stack([x.norm_3.weight.detach() for x in lay])
+        with torch.inference_mode():
+            self._adapters[name] = pack_adapter(lora, norm1, norm3, self.embedding_dim, self.device)
+        if self._handle is not None:
+            self._register_adapter(name)
+
+    def remove_adapter(self, name: str):
+        if name not in self._adapters:
+            raise KeyError(f"adapter {name!r} is not registered")
+        if name in self._adapter_ids:
+            _lib.check(_lib.lib().vnb_adapter_remove(self._handle, self._adapter_ids.pop(name)))
+        del self._adapters[name]
+
+    def adapters(self) -> list:
+        """Names of the registered adapters."""
+        return sorted(self._adapters)
+
+    def _register_adapter(self, name: str):
+        p = self._adapters[name]
+        if p["a_qkv"].device != self.device:
+            with torch.inference_mode():
+                p = self._adapters[name] = {k: v.to(self.device) for k, v in p.items()}
+        w = _lib.AdapterWeights(**{k: v.data_ptr() for k, v in p.items()})
+        i = C.c_int32()
+        _lib.check(_lib.lib().vnb_adapter_add(self._handle, C.byref(w), C.byref(i)))
+        self._adapter_ids[name] = i.value
+
+    def _adapter_id(self, name) -> int:
+        """-1 for the base model, else the live handle's id of a registered adapter (raises for an unknown name)."""
+        if name is None:
+            return -1
+        if name not in self._adapters:
+            raise KeyError(f"adapter {name!r} is not registered (add_adapter; a hot swap of the base drops adapters)")
+        return self._adapter_ids[name]
 
     @torch.no_grad()
     def repack(self):
@@ -417,6 +559,8 @@ class VampNet(nn.Module):
             _lib.check(lib.vnb_model_create(C.byref(cfg), C.byref(w), C.byref(h)))
         self._handle, self._packed, self._packed_key = h, p, key
         self._packed_codec = codec
+        for name in self._adapters:
+            self._register_adapter(name)
 
     # ------------------------------------------------------------------ forward
     class _NoCodec:
@@ -452,16 +596,24 @@ class VampNet(nn.Module):
         return logits.permute(0, 2, 1)
 
     @torch.no_grad()
-    def forward_codes(self, codes: torch.Tensor, codec) -> torch.Tensor:
-        """embedding.from_codes + forward fused: codes (B, C, T) int64 (mask token allowed) -> (B, S, V) fp32."""
+    def forward_codes(self, codes: torch.Tensor, codec, adapter: str = None) -> torch.Tensor:
+        """embedding.from_codes + forward fused: codes (B, C, T) int64 (mask token allowed) -> (B, S, V) fp32.
+        adapter: the name of a registered adapter (add_adapter) to apply, None for the base model."""
+        if adapter is not None and adapter not in self._adapters:
+            self._adapter_id(adapter)  # raises
         self._ensure_handle(codec)
         B, C_, T = codes.shape
         assert C_ == self.n_codebooks
         codes = codes.to(self.device, torch.int64).contiguous()
         logits = torch.empty(B, T * self.n_predict_codebooks, self.vocab_size, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().vnb_forward_codes(self._handle, _lib.ptr(codes), B, T, _lib.ptr(logits),
-                                                    _lib.stream_ptr(self.device)))
+            if adapter is None:
+                _lib.check(_lib.lib().vnb_forward_codes(self._handle, _lib.ptr(codes), B, T, _lib.ptr(logits),
+                                                        _lib.stream_ptr(self.device)))
+            else:
+                rows = (C.c_int32 * B)(*([self._adapter_id(adapter)] * B))
+                _lib.check(_lib.lib().vnb_forward_codes_adapted(self._handle, _lib.ptr(codes), B, T, rows,
+                                                                _lib.ptr(logits), _lib.stream_ptr(self.device)))
         return logits
 
     def hidden_state(self, B: int, T: int) -> torch.Tensor:
@@ -497,6 +649,7 @@ class VampNet(nn.Module):
         cfg_guidance: float = None,
         cond=None,
         philox_key: int = None,
+        adapter: str = None,
     ):
         """Iterative parallel decoding, reference transformer.py:686-946.
 
@@ -506,10 +659,12 @@ class VampNet(nn.Module):
         doubles the batch; it is None on every call path of Interface and is rejected here.
         philox_key (not in the reference): a key already drawn with draw_philox_key(); the global RNGs are then left
         alone, and `seed` must be None.
+        adapter (not in the reference): the name of a registered adapter (add_adapter) to generate with, None for the
+        base model.
         """
         call = self._prepare_call(codec, time_steps, _sampling_steps, start_tokens, temperature, mask,
                                   mask_temperature, ctrls, ctrl_masks, top_p, seed, sample_cutoff, cfg_guidance,
-                                  philox_key)
+                                  philox_key, adapter)
         out = self._launch_calls([call])[0]
         if return_signal:
             return self.decode(out, codec)
@@ -523,8 +678,8 @@ class VampNet(nn.Module):
         [self.generate(codec, **c) for c in calls] bit for bit, return_signal included, and the random, numpy and torch
         global RNG states afterwards are those the sequential calls leave: keys are drawn (draw_philox_key) in list
         order.  Calls with the same T, sampling steps and top-p on/off share one vnb_generate_many launch, in which
-        each keeps its own N0, temperatures, schedules, top_p and key; a launch whose B*T would exceed MANY_MAX_ROWS is
-        split."""
+        each keeps its own N0, temperatures, schedules, top_p, key and adapter; a launch whose B*T would exceed
+        MANY_MAX_ROWS is split."""
         import inspect
         sig = inspect.signature(VampNet.generate)
         prepared, want_signal = [], []
@@ -535,14 +690,16 @@ class VampNet(nn.Module):
             prepared.append(self._prepare_call(codec, a["time_steps"], a["_sampling_steps"], a["start_tokens"],
                                                a["temperature"], a["mask"], a["mask_temperature"], a["ctrls"],
                                                a["ctrl_masks"], a["top_p"], a["seed"], a["sample_cutoff"],
-                                               a["cfg_guidance"], a["philox_key"]))
+                                               a["cfg_guidance"], a["philox_key"], a["adapter"]))
             want_signal.append(bool(a["return_signal"]))
         outs = self._launch_calls(prepared)
         return [self.decode(o, codec) if sig_ else o for o, sig_ in zip(outs, want_signal)]
 
     def _prepare_call(self, codec, time_steps, steps, start_tokens, temperature, mask, mask_temperature, ctrls,
-                      ctrl_masks, top_p, seed, sample_cutoff, cfg_guidance, philox_key) -> dict:
+                      ctrl_masks, top_p, seed, sample_cutoff, cfg_guidance, philox_key, adapter=None) -> dict:
         """Validate one generate() call, draw its key and stage its device inputs and per-step host schedules."""
+        if adapter is not None and adapter not in self._adapters:
+            self._adapter_id(adapter)  # raises before any RNG is touched
         if ctrls is not None or ctrl_masks is not None:
             raise NotImplementedError("ctrls/ctrl_masks: ControlEncoder is outside the hot path")
         if cfg_guidance is not None:
@@ -573,7 +730,7 @@ class VampNet(nn.Module):
         return dict(z=z, mask=m32, steps=steps, temperature=float(temperature), gamma=[float(v) for v in g],
                     temp_eff=[float(v) for v in temp_eff],
                     do_sample=[1 if (i / steps) <= sample_cutoff else 0 for i in range(steps)], key=k,
-                    top_p=float(top_p) if (top_p is not None and top_p < 1.0) else 0.0)
+                    top_p=float(top_p) if (top_p is not None and top_p < 1.0) else 0.0, adapter=adapter)
 
     def _launch_calls(self, calls: list) -> list:
         """Launch prepared calls, one vnb_generate_many per (T, steps, top-p on) bucket of at most MANY_MAX_ROWS rows
@@ -627,11 +784,17 @@ class VampNet(nn.Module):
             g.rows, g.temperature, g.temp_eff, g.do_sample = c["z"].shape[0], c["temperature"], tef, dos
             g.seed_lo, g.seed_hi, g.top_p = c["key"] & 0xFFFFFFFF, (c["key"] >> 32) & 0xFFFFFFFF, c["top_p"]
         gam = (C.c_float * steps)(*calls[0]["gamma"])
+        ids = [self._adapter_id(c.get("adapter")) for c in calls]
         out = torch.empty_like(z)
+        graph = 1 if self.use_cuda_graph else 0
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().vnb_generate_many(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam, groups,
-                                                    len(calls), 1 if self.use_cuda_graph else 0, _lib.ptr(out),
-                                                    _lib.stream_ptr(dev)))
+            if any(i >= 0 for i in ids):
+                _lib.check(_lib.lib().vnb_generate_many_adapted(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps,
+                                                                gam, groups, len(calls), (C.c_int32 * len(calls))(*ids),
+                                                                graph, _lib.ptr(out), _lib.stream_ptr(dev)))
+            else:  # no call has an adapter: the plain kernels and graph
+                _lib.check(_lib.lib().vnb_generate_many(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam,
+                                                        groups, len(calls), graph, _lib.ptr(out), _lib.stream_ptr(dev)))
         keep.append((z, m32, out))
         return list(out.split([c["z"].shape[0] for c in calls]))
 
