@@ -265,6 +265,33 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
                             int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token, float temperature,
                             int32_t do_sample, int32_t step, uint32_t seed_lo, uint32_t seed_hi, void* partials,
                             void* stream);
+/* Test-only: one sampling step of the generate loop alone, with everything vnb_generate_many gives it made explicit.
+ * A group is `rows` consecutive batch rows with the scalars of one generate() call at one step (fields as in
+ * vnb_gen_group and vnb_gen_params; gamma = the schedule value of this step, is_last = this is the last step). */
+typedef struct vnb_sample_group {
+  int32_t rows;
+  float temperature; /* <= 0 means 1 */
+  float gamma, temp_eff;
+  int32_t do_sample, is_last, step;
+  uint32_t seed_lo, seed_hi;
+  float top_p; /* <= 0 or >= 1: no nucleus filter */
+} vnb_sample_group;
+/* path 0: sample_rows_kernel (no nucleus filter) on logits, then the re-mask;
+ * path 1: sample_rows_kernel with the nucleus filter (groups whose top_p is disabled draw as in path 0), then the
+ *         re-mask;
+ * path 2: sample_combine_kernel on caller-supplied partials (the records vnb_dbg_gemm_sample writes, row m = b*T + t),
+ *         then the re-mask;
+ * path 3: the re-mask alone, on caller-supplied tokens and conf.
+ * logits (B*S, V) fp32 (paths 0, 1), S = T * (C - ncc); partials (B*S*V/128) float4 (path 2); zcur (B, T, C) int32,
+ * updated in place; zorig (B, T, C) int32 or NULL (then the conditioning codebooks of zcur are left as they are);
+ * tokens, conf (B, S) written by paths 0-2, read by path 3; n0 DEVICE [n_groups] initial mask count of each group.
+ * The [group] table of sampling scalars and the row -> group map are built as vnb_generate_many builds them (the Philox
+ * counter of batch row b uses b minus its group's first row).  Refused: path outside 0..3, B or T < 1, ncc outside
+ * 0..C-1, V not a multiple of 128 in 128..1024, group rows that do not sum to B (or n_groups outside 1..B), a NULL buffer
+ * the path needs.  Synchronises `stream` before returning (the staged table is freed). */
+int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                       int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
+                       int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream);
 
 /* ---- codec (DAC family; reference call sites: interface.py:223 codec.encode, transformer.py:671-675
  *      codec.quantizer.from_latents + codec.decode).  fp32, (B, C, T) channels-first. ------------------------

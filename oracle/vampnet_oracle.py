@@ -335,7 +335,8 @@ class OracleVampNet:
             assert V % TILE == 0
             xs = (logits.numpy().astype(np.float32) * inv_t).reshape(B, S, V // TILE, TILE)
             m_k = xs.max(-1)                                                        # tile maxima
-            e = np.exp(xs - m_k[..., None], dtype=np.float32)
+            # a tile the nucleus filter emptied (all -inf) has mass 0, not exp(-inf - -inf) = NaN
+            e = np.exp(xs - np.where(np.isfinite(m_k), m_k, 0.0)[..., None], dtype=np.float32)
             cdf_in = np.cumsum(e, axis=-1, dtype=np.float32)                        # within-tile, sequential fp32
             mass = cdf_in[..., -1] * np.exp(m_k - m_k.max(-1, keepdims=True), dtype=np.float32)
             cdf_t = np.cumsum(mass, axis=-1, dtype=np.float32)

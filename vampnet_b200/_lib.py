@@ -51,6 +51,14 @@ class GenGroup(C.Structure):
     ]
 
 
+class SampleGroup(C.Structure):
+    _fields_ = [
+        ("rows", C.c_int32), ("temperature", C.c_float), ("gamma", C.c_float), ("temp_eff", C.c_float),
+        ("do_sample", C.c_int32), ("is_last", C.c_int32), ("step", C.c_int32), ("seed_lo", C.c_uint32),
+        ("seed_hi", C.c_uint32), ("top_p", C.c_float),
+    ]
+
+
 _SIGS = {
     "vnb_abi_version": (C.c_int32, []),
     "vnb_last_error": (C.c_char_p, []),
@@ -107,6 +115,8 @@ _SIGS = {
                                         C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,
                                         C.c_void_p, C.c_void_p]),
+    "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
+                                                                                        C.c_int32, C.c_void_p]),
 }
 
 _lib = None

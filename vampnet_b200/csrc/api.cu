@@ -896,5 +896,55 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
   CK(launch_gemm(p, st));
   return 0;
 }
+int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                       int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
+                       int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream) {
+  if (path < 0 || path > 3) return fail("vnb_dbg_sample: path %d outside 0..3", path);
+  if (B < 1 || T < 1 || ncc < 0 || C <= ncc) return fail("vnb_dbg_sample: need B >= 1, T >= 1 and 0 <= ncc < C");
+  if (V % 128 != 0 || V < 128 || V > 1024) return fail("vnb_dbg_sample: need V %% 128 == 0, 128 <= V <= 1024 (got %d)", V);
+  if (!zcur || !tokens || !conf || !n0 || !groups) return fail("vnb_dbg_sample: zcur, tokens, conf, n0 and groups are required");
+  if (path <= 1 && !logits) return fail("vnb_dbg_sample: path %d needs logits", path);
+  if (path == 2 && !partials) return fail("vnb_dbg_sample: path 2 needs partials");
+  if (n_groups < 1 || n_groups > B) return fail("vnb_dbg_sample: n_groups %d out of range 1..B (B = %d)", n_groups, B);
+  long long total = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    if (groups[g].rows < 1) return fail("vnb_dbg_sample: group %d has %d rows", g, groups[g].rows);
+    total += groups[g].rows;
+  }
+  if (total != B) return fail("vnb_dbg_sample: group rows sum to %lld, not B = %d", total, B);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // one step's row of the [step][group] table and the row map, as vnb_generate_many_adapted fills them
+  std::vector<SampleDyn> dyn(n_groups);
+  std::vector<RowGroup> rowgrp(B);
+  for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
+    const vnb_sample_group& q = groups[g];
+    SampleDyn& d = dyn[g];
+    d.inv_temp = inv_temperature(q.temperature);
+    d.gamma = q.gamma;
+    d.temp_eff = q.temp_eff;
+    d.do_sample = q.do_sample;
+    d.is_last = q.is_last;
+    d.step = q.step;
+    d.seed_lo = q.seed_lo;
+    d.seed_hi = q.seed_hi;
+    d.top_p = q.top_p;
+    for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
+  }
+  DevBuf dyn_dev, grp_dev;
+  CK(dyn_dev.alloc(sizeof(SampleDyn) * n_groups));
+  CK(grp_dev.alloc(sizeof(RowGroup) * B));
+  CK(cudaMemcpyAsync(dyn_dev.p, dyn.data(), sizeof(SampleDyn) * n_groups, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+  SampleArgs sa;
+  sa.logits = logits; sa.zcur = zcur; sa.zorig = zorig; sa.tokens = tokens; sa.conf = conf; sa.n0 = n0;
+  sa.rowgrp = grp_dev.as<RowGroup>();
+  sa.B = B; sa.T = T; sa.C = C; sa.ncc = ncc; sa.V = V; sa.mask_token = mask_token;
+  const SampleDyn* dd = dyn_dev.as<SampleDyn>();
+  if (path <= 1) CK(launch_sample_step_dev(sa, dd, st, path == 1));
+  else if (path == 2) CK(launch_sample_combine_dev(sa, partials, dd, st));
+  else CK(launch_remask_dev(sa, dd, st));
+  CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
+  return 0;
+}
 
 }  // extern "C"

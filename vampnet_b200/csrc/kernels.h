@@ -158,5 +158,7 @@ struct SampleArgs {
 cudaError_t launch_sample_step_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st, bool use_top_p);
 // fused path: the classifier's sampling epilogue wrote `partials`; picks the tile, writes tokens + confidences, re-masks
 cudaError_t launch_sample_combine_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
+// the re-mask alone (the second kernel of both launchers above): reads a.tokens and a.conf, updates a.zcur
+cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st);
 
 }  // namespace vnb

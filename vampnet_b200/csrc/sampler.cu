@@ -80,6 +80,12 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
   // first token over the threshold).  Equivalent per-token rule: keep v iff sum_{u: x_u > x_v} p_u <= top_p.
   // The smallest kept key is found by bisection over the order-preserving uint image of the floats.
   if (TOPP && dyn.top_p > 0.f && dyn.top_p < 1.f) {
+    // +0 and -0 are one logit value (a tie, kept or dropped whole) but have different keys: make every zero +0.  No
+    // other use of x can tell the two apart.
+#pragma unroll
+    for (int i = 0; i < MAXV4; ++i) {
+      if (i < n4) { x[i].x += 0.f; x[i].y += 0.f; x[i].z += 0.f; x[i].w += 0.f; }
+    }
     const float gm = warp_max(mx);
     float pr[MAXV4 * 4];
     float ps = 0.f;
@@ -406,6 +412,11 @@ static SampleStatic make_static(const SampleArgs& s) {
   return a;
 }
 
+cudaError_t launch_remask_dev(const SampleArgs& s, const SampleDyn* dyn_dev, cudaStream_t st) {
+  remask_kernel<<<s.B, 1024, 0, st>>>(make_static(s), dyn_dev);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_sample_step_dev(const SampleArgs& s, const SampleDyn* dyn_dev, cudaStream_t st, bool use_top_p) {
   const SampleStatic a = make_static(s);
   if (s.V % 128 != 0 || s.V > 1024) return cudaErrorInvalidValue;
@@ -414,8 +425,7 @@ cudaError_t launch_sample_step_dev(const SampleArgs& s, const SampleDyn* dyn_dev
   else sample_rows_kernel<false><<<(rows + 7) / 8, 256, 0, st>>>(a, dyn_dev);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  remask_kernel<<<s.B, 1024, 0, st>>>(a, dyn_dev);
-  return cudaGetLastError();
+  return launch_remask_dev(s, dyn_dev, st);
 }
 
 cudaError_t launch_sample_combine_dev(const SampleArgs& s, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st) {
@@ -425,8 +435,7 @@ cudaError_t launch_sample_combine_dev(const SampleArgs& s, const void* partials,
   sample_combine_kernel<<<(rows + 255) / 256, 256, 0, st>>>(a, reinterpret_cast<const float4*>(partials), dyn_dev);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  remask_kernel<<<s.B, 1024, 0, st>>>(a, dyn_dev);
-  return cudaGetLastError();
+  return launch_remask_dev(s, dyn_dev, st);
 }
 
 }  // namespace vnb
