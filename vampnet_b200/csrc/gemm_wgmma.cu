@@ -15,6 +15,8 @@
 //                accumulators per thread; then the epilogue: the accumulators go to a padded fp32 tile that overlays the
 //                drained ring, and each epilogue warp reads 32 x 32 chunks of it in store order -> fused op -> global
 //                (4 warps; 8 for the residual and the sampling epilogues)
+// The FFN-up GEMM without adapters runs gemm_geglu_persistent_kernel instead: the same mainloop in one CTA per SM, with
+// each tile's stores overlapping the next tile's MMAs.
 //
 // Roofline: tensor-bound.  Algorithmic work = 2*M*N*K flop per launch; bytes (A+W+out) are a few
 // MB against > 10 GFLOP, far right of the ridge.
@@ -78,6 +80,18 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   const float e = __expf(2.0f * y);
   const float t = 1.0f - __fdividef(2.0f, 1.0f + e);
   return 0.5f * x * (1.0f + t);
+}
+
+// Row scale of the fused RMSNorm of the A operand: rsqrt(mean(x^2) + eps) of output row `row`, from the partial sums of
+// squares in a fixed order; 1 without a fused norm and past M.
+__device__ __forceinline__ float row_scale(const GemmArgs& g, int row) {
+  float rs = 1.0f;
+  if (g.ss_in != nullptr && row < g.M) {
+    float t = 0.f;
+    for (int p = 0; p < g.ss_parts; ++p) t += __ldg(g.ss_in + static_cast<size_t>(p) * g.M + row);
+    rs = rsqrtf(t * g.inv_d + g.eps);
+  }
+  return rs;
 }
 
 // ---- epilogue ---------------------------------------------------------------------------------
@@ -246,6 +260,34 @@ __device__ __forceinline__ void lora_update(const GemmArgs& g, uint8_t* scratch,
   }
 }
 
+// The k-block loop of one tile (consumer warpgroup `wg`, rows [64 wg, 64 wg + 64)): acc += A W^T over every k-block in
+// order, 4 x k16 per 64-wide k-block.  `stage` / `phase` are the ring position of the first k-block and are left at
+// the one after the last, so a persistent CTA continues the ring from tile to tile.  release(s) hands stage s back to
+// the producer once the MMAs reading it have retired.
+template <typename Release>
+__device__ __forceinline__ void gemm_mainloop(float (&acc)[128], uint8_t* ring, uint64_t* full_bar, int num_kb, int wg,
+                                              int& stage, uint32_t& phase, Release&& release) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(ring + stage * STAGE_BYTES) + wg * (64 * 128);
+    const uint32_t sb = smem_u32(ring + stage * STAGE_BYTES + A_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)  // advance 16 bf16 = 32 B along K inside the 128B swizzle span
+      wgmma_ss_n256(acc, wgmma_desc_sw128(sa + k * 32), wgmma_desc_sw128(sb + k * 32), 1u);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+    wgmma_fence_regs(acc);
+    if (kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  if (num_kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
+}
+
 // PAIR = true: clusters of two CTAs on vertically adjacent 128 x 256 tiles (the same 256 W rows).  Each CTA fetches
 // half of the W tile (128 rows) and the TMA multicasts it into both CTAs' shared memory, so per CTA the W bytes pulled
 // from L2 are halved; a stage is refilled only when the consumer warps of both CTAs have released it.  Every output
@@ -313,34 +355,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int wg = warp >> 2;
     {
       float acc[128];
-#pragma unroll
-      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
       const uint32_t peer_empty = PAIR ? mapa_u32(smem_u32(empty_bar), rank ^ 1u) : 0u;
-      auto release = [&](int s) {
+      int stage = 0;
+      uint32_t phase = 0;
+      gemm_mainloop(acc, smem, full_bar, num_kb, wg, stage, phase, [&](int s) {
         if (lane == 0) {
           mbar_arrive(&empty_bar[s]);
           if constexpr (PAIR) mbar_arrive_cluster(peer_empty + 8u * s);
         }
-      };
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * (64 * 128);
-        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // advance 16 bf16 = 32 B along K inside the 128B swizzle span
-          wgmma_ss_n256(acc, wgmma_desc_sw128(sa + k * 32), wgmma_desc_sw128(sb + k * 32), 1u);
-        wgmma_commit();
-        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
-        wgmma_fence_regs(acc);
-        if (kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc);
-      if (num_kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
+      });
       // both warpgroups are done reading the ring (every TMA write into it has landed: all full barriers were waited
       // on); the accumulators go to the fp32 tile that overlays it.  Fragment of m64nNk16: thread (warp w, lane l)
       // holds rows 16 w + l/4 and + 8, columns 8 i + 2 (l % 4) + {0, 1}.
@@ -374,12 +397,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       const int half = kWide ? (warp >> 2) : 0;  // 8-warp epilogue: this warp takes chunks with (c & 1) == half
       const int row_base = m0 + quad * 32;
-      float rs = 1.0f;  // fused RMSNorm of the A operand: rsqrt(mean(x^2) + eps) of this thread's row
-      if (g.ss_in != nullptr && row_ok) {
-        float t = 0.f;
-        for (int p = 0; p < g.ss_parts; ++p) t += __ldg(g.ss_in + static_cast<size_t>(p) * g.M + row);
-        rs = rsqrtf(t * g.inv_d + g.eps);
-      }
+      const float rs = row_scale(g, row);  // fused RMSNorm of the A operand, this thread's row
       // this warp's quadrant of the accumulator tile, and this thread's row in it (column c at t_addr + 4 c)
       const uint32_t qaddr = smem_u32(smem) + 4u * (quad * 32 * ACC_PITCH);
       const uint32_t t_addr = qaddr + 4u * (lane * ACC_PITCH);
@@ -551,6 +569,140 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if constexpr (PAIR) cluster_sync_all();
 }
 
+// Persistent FFN-up GEMM (GEGLU, no adapters): one CTA per SM walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ...
+// in the same n-fastest order, and a tile's stores run on dedicated warps while the consumers compute the next tile.
+//   warp 11      TMA producer: the same 4-stage ring as gemm_wgmma_kernel, continued across tile boundaries
+//   warps 0..7   consumers: the same mainloop; then value * gelu_tanh(gate) in registers (value column c and gate column
+//                c + 128 are fragments i and i + 16 of the same thread), rounded to bf16 into the staging tile
+//   warps 8..10  epilogue: copy the staging tile to global memory in whole rows, then compute the row scales of the
+//                CTA's next tile into shared memory
+// Handing over only the 128 x 128 bf16 result (32 KiB) leaves room for the full ring.  Per output element the operands,
+// the k order, the accumulator and the arithmetic (row scale, GEGLU, rounding) are those of gemm_wgmma_kernel's GEGLU
+// epilogue: bit-identical.
+constexpr int GG_EPI_WARPS = 3;
+constexpr int GG_THREADS = 256 + 32 * GG_EPI_WARPS + 32;  // 384: ptxas sizes registers per SM sub-partition, a 13th
+                                                          // warp would cap every thread at 128
+constexpr int GG_STAGE_BYTES = BM * (BN / 2) * 2;  // bf16 result tile, rows of 256 B, 16-byte units XOR-swizzled by row
+constexpr int GG_SMEM = RING_BYTES + GG_STAGE_BYTES + 4 * BM /*row scales*/ + 1024 /*align slack*/ + 128 /*barriers*/;
+static_assert(GG_SMEM <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
+static_assert((2 * STAGES + 2) * 8 <= 128, "the barriers fit their slot");
+
+// byte offset of the 4-byte word holding result columns (2 w, 2 w + 1) of tile row r in the staging tile: the 16-byte
+// unit w / 4 is XORed with r % 8, so the consumers' fragment stores (8 rows x 4 words) and the epilogue's row reads
+// (8 consecutive units of one row) are both bank-conflict free
+__device__ __forceinline__ uint32_t gg_stage_off(int r, int w) {
+  return static_cast<uint32_t>(r * 256 + (((w >> 2) ^ (r & 7)) << 4) + ((w & 3) << 2));
+}
+
+__global__ void __launch_bounds__(GG_THREADS, 1)
+gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                             const GemmArgs g) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t stage_tile = smem_u32(smem + RING_BYTES);
+  float* srs = reinterpret_cast<float*>(smem + RING_BYTES + GG_STAGE_BYTES);  // row scales of the tile being computed
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING_BYTES + GG_STAGE_BYTES + 4 * BM);
+  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* out_full = empty_bar + STAGES;  // the staging tile holds a result tile (256 consumer threads)
+  uint64_t* out_free = out_full + 1;        // the staging tile is free and srs holds the next tile's row scales
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_n = g.N / BN;
+  const int num_kb = g.K / BK;
+  const int tiles = ((g.M + BM - 1) / BM) * num_n;
+  constexpr int kProducer = 8 + GG_EPI_WARPS;
+
+  if (warp == kProducer && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // lane 0 of every consumer warp
+    }
+    mbar_init(out_full, 256);
+    mbar_init(out_free, 32 * GG_EPI_WARPS);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp == kProducer) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+          tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m0);
+          tma_load_2d(sa + A_BYTES, &tmB, &full_bar[stage], kb * BK, n0);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    __syncwarp();
+  } else if (warp < 8) {
+    // ===================== consumers =====================
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t it = 0;
+    // fragment of m64nNk16: thread (warp w, lane l) holds rows 16 w + l/4 and + 8, columns 8 i + 2 (l % 4) + {0, 1}
+    const int r = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
+      float acc[128];
+      gemm_mainloop(acc, smem, full_bar, num_kb, warp >> 2, stage, phase, [&](int s) {
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+      });
+      mbar_wait(out_free, it & 1u);  // the previous result tile is stored, srs holds this tile's row scales
+      const float rs0 = srs[r], rs1 = srs[r + 8];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        float x[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float rsr = k < 2 ? rs0 : rs1;
+          x[k] = acc[4 * i + k] * rsr;
+          x[k] = x[k] * gelu_tanh(acc[4 * (i + 16) + k] * rsr);
+        }
+        const int w = 4 * i + (lane & 3);
+        sts_u32(stage_tile + gg_stage_off(r, w), pack_bf16x2(x[0], x[1]));
+        sts_u32(stage_tile + gg_stage_off(r + 8, w), pack_bf16x2(x[2], x[3]));
+      }
+      mbar_arrive(out_full);
+    }
+  } else {
+    // ===================== epilogue =====================
+    const int e = warp - 8;
+    __nv_bfloat16* const out = reinterpret_cast<__nv_bfloat16*>(g.out);
+    const int pitch = g.N / 2;
+    auto row_scales = [&](int tile) {  // row scales of `tile` into srs, then hand the staging tile to the consumers
+      if (tile < tiles) {
+        const int m0 = (tile / num_n) * BM;
+        for (int j = e * 32 + lane; j < BM; j += 32 * GG_EPI_WARPS) srs[j] = row_scale(g, m0 + j);
+      }
+      mbar_arrive(out_free);
+    };
+    row_scales(blockIdx.x);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
+      const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
+      mbar_wait(out_full, it & 1u);
+      // two tile rows per warp instruction: lane -> (row 2 u + lane / 16, 16-byte unit lane % 16)
+#pragma unroll 4
+      for (int u = e; u < BM / 2; u += GG_EPI_WARPS) {
+        const int rr = 2 * u + (lane >> 4);
+        const float4 v = lds_f4(stage_tile + gg_stage_off(rr, 4 * (lane & 15)));
+        if (m0 + rr < g.M)
+          *reinterpret_cast<float4*>(out + static_cast<size_t>(m0 + rr) * pitch + (n0 >> 1) + 8 * (lane & 15)) = v;
+      }
+      row_scales(tile + gridDim.x);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Single-CTA tiles or clusters of two CTAs sharing the W tile: vnb_set_option("gemm_pair", 0|1), else the environment
 // variable VNB_GEMM_PAIR, else the compiled default.
@@ -582,6 +734,10 @@ static cudaError_t init_epi() {
     e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
+    if (e != cudaSuccess) return e;
+  }
+  if constexpr (EPI == VNB_EPI_GEGLU) {
+    e = cudaFuncSetAttribute(gemm_geglu_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GG_SMEM);
     if (e != cudaSuccess) return e;
   }
   cudaLaunchConfig_t q = {};
@@ -616,7 +772,9 @@ int get_gemm_max_clusters() {
   return g_max_clusters[VNB_EPI_RESID][dev];
 }
 
-// One CTA per output tile (the accumulator tile overlays the operand ring, so a CTA does not start a second tile).
+// One CTA per output tile (the accumulator tile overlays the operand ring, so a CTA does not start a second tile), except
+// for the FFN-up GEMM without adapters: the persistent kernel, one CTA per SM (the SM count is cached by prepare_gemm(),
+// so none is queried inside a capture).
 template <int EPI, bool ADAPT = false>
 static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t st) {
   cudaError_t e = init_epi<EPI>();
@@ -635,6 +793,11 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
     return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true, ADAPT>, p.tmA, p.tmBh, g);
   }
   const int tiles = ((g.M + BM - 1) / BM) * (g.N / BN);
+  if constexpr (EPI == VNB_EPI_GEGLU && !ADAPT) {
+    const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
+    gemm_geglu_persistent_kernel<<<grid, GG_THREADS, GG_SMEM, st>>>(p.tmA, p.tmB, g);
+    return cudaGetLastError();
+  }
   gemm_wgmma_kernel<EPI, false, ADAPT><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
   return cudaGetLastError();
 }
