@@ -170,6 +170,20 @@ int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, i
 int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
                                   int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
                                   const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream);
+/* vnb_generate_many_adapted for calls of different lengths: group g is a call of group_frames[g] frames (host
+ * [n_groups], each in 1..T), padded to the launch's T.  Its rows' frames t >= group_frames[g] must be kept frames
+ * (mask 0) in z / mask; mask is then required.  Attention stops at each row's own length and the padded key columns
+ * are zero, so every group's first group_frames[g] frames of out equal, bit for bit, vnb_generate_many_adapted of
+ * its rows alone at T = group_frames[g]; its later frames of out are the padding's codes.  group_frames NULL, or every
+ * entry T: vnb_generate_many_adapted.  group_adapter may be NULL (all base).  A launch with a shorter group runs the
+ * frames-aware QKV and attention (one more graph per workspace key); the per-row frames table is written before
+ * every launch or replay and never causes a capture, so one (B, T) graph serves any mix of lengths.
+ * Errors: those of vnb_generate_many, a group_frames entry outside 1..T, and a NULL mask with a group shorter than T
+ * (the default mask would mask the padding). */
+int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                            const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                            const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
+                            void* stream);
 /* One sampling iteration on caller-supplied logits (B, S, V) fp32 — sample_from_logits +
  * mask_by_random_topk + the where()s around them (transformer.py:849-932).  State is explicit:
  * zflat (B, S) int32 in "t c" order (util.py:39) is updated in place; tokens_out (B, S) int32
@@ -184,8 +198,9 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
  * vnb_launch_count: kernels launched by this library so far in this process (a graph replay adds the
  * number of kernel nodes it contains).
  * vnb_graph_capture_count: generate graphs captured so far (a weight hot swap or a repeated call must not
- * add to it: graphs are cached per (workspace, steps, mask, top_p, adapted or not); the grouping of
- * vnb_generate_many and the group -> adapter table are not part of that key).
+ * add to it: graphs are cached per (workspace, steps, mask, top_p, adapted or not, some group shorter than T or
+ * not); the grouping of vnb_generate_many, the group -> adapter table and the per-row frames of vnb_generate_ragged
+ * are not part of that key).
  * vnb_profile_begin/end: between the two calls every launch of forward/generate is bracketed by CUDA
  * events on the launching stream (graph replay is bypassed so that the events can be recorded);
  * end() returns the summed device time and launch count per kernel family:
@@ -229,6 +244,12 @@ int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_
  * qk (B, T, 2d) bf16 [q | k], vT (B, d, Tpad) bf16, out (B, T, d) bf16, d = H*64. */
 int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                          int32_t B, int32_t T, int32_t Tpad, int32_t H, void* stream);
+/* Test-only: vnb_op_attention with a key length per batch row, frames DEVICE [B], entries in 1..T.  Row b attends to
+ * keys t < frames[b] only and writes out rows t < frames[b] only; its later rows of qk may hold anything, its later
+ * columns of vT must be zero (as the QKV epilogue of vnb_dbg_gemm_qkv_frames leaves them).  Query tiles wholly past
+ * frames[b] do no work. */
+int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
+                                 int32_t B, int32_t T, int32_t Tpad, int32_t H, const int32_t* frames, void* stream);
 /* Naive SIMT GEMM used only to bisect the tensor-core path in tests: out fp32 (M, N) = A x W^T. */
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream);
 /* Test-only: vnb_op_gemm plus the fused-RMSNorm plumbing the forward uses, epi in {BF16, QKV, RESID, GEGLU, BIAS_F32}.
@@ -252,6 +273,13 @@ int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t 
                              void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
                              float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
                              int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream);
+/* Test-only: the QKV GEMM of a launch of calls with different lengths: vnb_dbg_gemm_fused(VNB_EPI_QKV, ...) with
+ * adapters NULL, else vnb_dbg_gemm_adapted(VNB_EPI_QKV, ...), plus frames DEVICE [ceil(M / T)]: vT column t of batch
+ * row b is written as exactly 0 for t >= frames[b].  Everything else is what the call without frames writes. */
+int32_t vnb_dbg_gemm_qkv_frames(const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out, void* vT,
+                                int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d, float eps,
+                                const int32_t* frames, const vnb_adapter_weights* adapters, int32_t n_adapters,
+                                int32_t layer, const int32_t* row_adapter, float* u, void* stream);
 /* Test-only: the classifier GEMM with the sampling epilogue of the generate loop (VNB_EPI_SAMPLE) alone.
  * N == (C - ncc) * V, V % 128 == 0, V <= 1024; logits x = (A . W^T) * rs + bias with rs as above.
  * zcur (M, C) int32, row m = b*T + t: codebook ncc + cp of row m is sampled iff it holds mask_token.

@@ -77,6 +77,9 @@ _SIGS = {
     "vnb_generate_many_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                               C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32,
                                               C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_generate_ragged": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                        C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32, C.POINTER(C.c_int32),
+                                        C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_adapter_add": (C.c_int32, [C.c_void_p, C.POINTER(AdapterWeights), C.POINTER(C.c_int32)]),
     "vnb_adapter_remove": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vnb_forward_codes_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
@@ -94,6 +97,8 @@ _SIGS = {
                                 C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "vnb_op_attention": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_int32, C.c_int32, C.c_void_p]),
+    "vnb_dbg_attention_ragged": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                             C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_codec_conv1d": (C.c_int32, [C.c_void_p] * 6 + [C.c_int32] * 13 + [C.c_void_p]),
     "vnb_codec_rvq": (C.c_int32, [C.c_int32] + [C.c_void_p] * 11 + [C.c_int32] * 6 + [C.c_void_p] * 3),
     "vnb_codec_conv_tc": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
@@ -111,6 +116,10 @@ _SIGS = {
                                          C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float,
                                          C.c_float, C.c_void_p, C.c_void_p, C.POINTER(AdapterWeights), C.c_int32,
                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_dbg_gemm_qkv_frames": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float, C.c_float,
+                                            C.c_void_p, C.POINTER(AdapterWeights), C.c_int32, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
     "vnb_dbg_gemm_sample": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                         C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,

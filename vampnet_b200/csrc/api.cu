@@ -140,9 +140,10 @@ struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in w
   int variant;  // GEMM kernel variant baked into the graph (vnb_set_option "gemm_pair")
   bool fused;   // sampler fused into the classifier epilogue (vnb_set_option "fused_sampler")
   bool adapted;  // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
+  bool ragged;   // QKV and attention read the frames table (some group is shorter than T)
   bool operator<(const GraphKey& o) const {
-    return std::tie(steps, has_mask, top_p, variant, fused, adapted) <
-           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted);
+    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged) <
+           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged);
   }
 };
 
@@ -156,6 +157,9 @@ struct Workspace {
   // adapted launches: grp_adapter (B) = the adapter of every group (-1: base), rewritten before every launch or replay;
   // lora_u (M, 16) = the down-projection of the GEMM about to run
   DevBuf grp_adapter, lora_u;
+  // launches of calls with different lengths: frames (B) = the length of every batch row's call, rewritten before every
+  // launch or replay (read by the QKV epilogue and attention)
+  DevBuf frames;
   int embKp = 0;
   int ss_parts = 0;
   std::vector<GemmPlan> qkv, wo, up, down;
@@ -253,6 +257,7 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   CK(ws->dyn.alloc(sizeof(SampleDyn) * vnb_model::kMaxSteps * B));
   CK(ws->rowgrp.alloc(sizeof(RowGroup) * B));
   CK(ws->grp_adapter.alloc(sizeof(int32_t) * B));
+  CK(ws->frames.alloc(sizeof(int32_t) * B));
   CK(ws->lora_u.alloc(M * 16 * 4));
   CK(ws->z_in.alloc(M * c.n_codebooks * 8));
   CK(ws->mask_in.alloc(M * c.n_codebooks * 4));
@@ -349,16 +354,22 @@ static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int 
   return 0;
 }
 
-// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.
+// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  ragged: batch row b
+// is a call of ws->frames[b] frames; its later frames are padding that no earlier frame attends to.
 static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st, float* acts = nullptr,
-                     const SampleDyn* fused_dyn = nullptr, bool adapted = false) {
+                     const SampleDyn* fused_dyn = nullptr, bool adapted = false, bool ragged = false) {
   const vnb_config& c = m->cfg;
   // RMSNorm (transformer.py:43-58) is fused: norm weights are folded into wqkv / w1 / wcls at pack time, the
   // producers of x (embed, attn-out, ffn-down) also emit bf16(x) and per-row sums of squares, and the consumers
   // scale their accumulator rows by rsqrt(mean(x^2) + eps).
+  const int32_t* frames = ragged ? ws->frames.as<int32_t>() : nullptr;
+  AttnPlan attn = ws->attn;
+  attn.frames = frames;
   for (int l = 0; l < c.n_layers; ++l) {
-    if (run_lora_gemm(m, ws, ws->qkv[l], FAM_GEMM_QKV, adapted, LORA_QKV, l, ws->y.p, st)) return 1;
-    LAUNCH(FAM_ATTN, launch_attention(ws->attn, st));
+    GemmPlan qkv = ws->qkv[l];
+    qkv.frames = frames;
+    if (run_lora_gemm(m, ws, qkv, FAM_GEMM_QKV, adapted, LORA_QKV, l, ws->y.p, st)) return 1;
+    LAUNCH(FAM_ATTN, launch_attention(attn, st));
     if (run_lora_gemm(m, ws, ws->wo[l], FAM_GEMM_O, adapted, LORA_WO, l, ws->att.p, st) ||
         run_lora_gemm(m, ws, ws->up[l], FAM_GEMM_UP, adapted, LORA_W1, l, ws->y.p, st) ||
         run_lora_gemm(m, ws, ws->down[l], FAM_GEMM_DOWN, adapted, LORA_W2, l, ws->h.p, st))
@@ -572,7 +583,7 @@ static int fused_sampler_enabled() {
 }
 
 static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int steps, int64_t* out,
-                            cudaStream_t st, bool use_top_p, bool fused, bool adapted) {
+                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
   // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
@@ -591,10 +602,10 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
     if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
     const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
     if (fused) {
-      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted)) return 1;
+      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted, ragged)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
     } else {
-      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted)) return 1;
+      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted, ragged)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_step_dev(sa, dyn_i, st, use_top_p));
     }
     ++g_launches;  // sample step = two kernels
@@ -604,9 +615,10 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   return 0;
 }
 
-int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
-                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
+int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                            const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                            const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
+                            void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
   if (!gamma || !groups) return fail("vnb_generate_many: gamma and groups are required");
@@ -624,6 +636,15 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
     total += q.rows;
   }
   if (total != B) return fail("vnb_generate_many: group rows sum to %lld, not B = %d", total, B);
+  // a group shorter than T: its rows' later frames are padding (kept frames in z / mask) that attention never reads
+  bool ragged = false;
+  for (int g = 0; group_frames && g < n_groups; ++g) {
+    if (group_frames[g] < 1 || group_frames[g] > T)
+      return fail("vnb_generate_ragged: group %d has %d frames, outside 1..T (T = %d)", g, group_frames[g], T);
+    ragged |= group_frames[g] < T;
+  }
+  // without a mask every predicted codebook is masked, padding included: it would be sampled and count in N0
+  if (ragged && !mask) return fail("vnb_generate_ragged: a launch with groups shorter than T needs a mask");
   if (check_adapter_ids(m, group_adapter, n_groups, "vnb_generate_many_adapted")) return 1;
   const bool adapted = any_adapted(group_adapter, n_groups);
   Workspace* ws;
@@ -633,6 +654,7 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
   // returning, so the vectors may die at scope exit
   std::vector<SampleDyn> dyn(static_cast<size_t>(steps) * B);
   std::vector<RowGroup> rowgrp(B);
+  std::vector<int32_t> frames(ragged ? B : 0);
   for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
     const vnb_gen_group& q = groups[g];
     const float inv_t = inv_temperature(q.temperature);
@@ -649,14 +671,16 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
       d.top_p = q.top_p;
     }
     for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
+    for (int b = first; ragged && b < first + q.rows; ++b) frames[b] = group_frames[g];
   }
   CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * dyn.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+  if (ragged) CK(cudaMemcpyAsync(ws->frames.p, frames.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
   if (adapted && stage_adapters(m, ws, group_adapter, n_groups, st)) return 1;
   const bool fused = fused_sampler_enabled() != 0 && !use_top_p && ws->can_fuse;
   if (!fused && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
-  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted);
+  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged);
 
   const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
   CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
@@ -664,7 +688,7 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
   const int64_t* gz = ws->z_in.as<int64_t>();
   const int32_t* gmask = mask ? ws->mask_in.as<int32_t>() : nullptr;
   int64_t* gout = ws->z_out.as<int64_t>();
-  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted};
+  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged};
   auto it = ws->graphs.find(key);
   if (it == ws->graphs.end()) {
     cudaStream_t cap;
@@ -673,7 +697,7 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cap); return fail("begin capture: %s", cudaGetErrorString(e)); }
     const unsigned long long before = g_launches;
-    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted);
+    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged);
     const unsigned long long in_graph = g_launches - before;
     g_launches = before;
     e = cudaStreamEndCapture(cap, &graph);
@@ -697,6 +721,14 @@ int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t*
   g_launches += ws->graph_kernels[key];
   CK(cudaMemcpyAsync(out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// Calls of one length are the group_frames = NULL case.
+int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
+  return vnb_generate_ragged(m, z, mask, B, T, steps, gamma, groups, n_groups, nullptr, group_adapter, use_graph, out,
+                             stream);
 }
 
 int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
@@ -804,6 +836,15 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
   CK(launch_attention(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
+int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
+                                 int32_t B, int32_t T, int32_t Tpad, int32_t H, const int32_t* frames, void* stream) {
+  if (!frames) return fail("vnb_dbg_attention_ragged: frames is required");
+  AttnPlan p;
+  if (!make_attn_plan(&p, qk, vT, out, rel_bias, rel_sat, B, T, Tpad, H)) return fail("attn plan: %s", tmap_error());
+  p.frames = frames;
+  CK(launch_attention(p, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream) {
   CK(launch_gemm_ref(A, W, M, N, K, out, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
@@ -829,10 +870,14 @@ int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M,
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
-int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
-                             void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
-                             float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
-                             int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
+}  // extern "C"
+
+// vnb_dbg_gemm_adapted, and (frames non-null) the adapted QKV of vnb_dbg_gemm_qkv_frames
+static int dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                            void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
+                            float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
+                            int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u,
+                            const int32_t* frames, void* stream) {
   if (epi != VNB_EPI_QKV && epi != VNB_EPI_RESID && epi != VNB_EPI_GEGLU)
     return fail("vnb_dbg_gemm_adapted: epilogue %d has no adapted variant", epi);
   if (!adapters || n_adapters < 1 || n_adapters > VNB_MAX_ADAPTERS || !row_adapter || !u || layer < 0)
@@ -869,9 +914,39 @@ int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t 
   p.lora.slot = epi == VNB_EPI_QKV ? LORA_QKV : epi == VNB_EPI_GEGLU ? LORA_W1 : (K == N ? LORA_WO : LORA_W2);
   p.lora.layer = layer;
   p.lora.u = u;
+  p.frames = frames;
   CK(launch_lora_down(A, M, K, p.lora, st));
   CK(launch_gemm(p, st));
   CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
+  return 0;
+}
+
+extern "C" {
+
+int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
+                             void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
+                             float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
+                             int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
+  return dbg_gemm_adapted(epi, A, W, M, N, K, out, out2, T, Tpad, ss_in, ss_parts, inv_d, eps, out_bf16, ss_out,
+                          adapters, n_adapters, layer, row_adapter, u, nullptr, stream);
+}
+int32_t vnb_dbg_gemm_qkv_frames(const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out, void* vT,
+                                int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d, float eps,
+                                const int32_t* frames, const vnb_adapter_weights* adapters, int32_t n_adapters,
+                                int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
+  if (!frames) return fail("vnb_dbg_gemm_qkv_frames: frames is required");
+  if (adapters)
+    return dbg_gemm_adapted(VNB_EPI_QKV, A, W, M, N, K, out, vT, T, Tpad, ss_in, ss_parts, inv_d, eps, nullptr,
+                            nullptr, adapters, n_adapters, layer, row_adapter, u, frames, stream);
+  if (vT == nullptr || N % 96 != 0 || T < 1 || Tpad < T)
+    return fail("vnb_dbg_gemm_qkv_frames: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
+  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_qkv_frames: ss_parts must be >= 1");
+  GemmPlan p;
+  if (!make_gemm_plan(&p, VNB_EPI_QKV, A, W, M, N, K, out, vT, nullptr, T, Tpad, (N / 3) * 2))
+    return fail("gemm plan: %s", tmap_error());
+  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
+  p.frames = frames;
+  CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,

@@ -10,7 +10,7 @@
 //   warp 8      TMA producer: Q once; K_j and V^T_j through a 3-stage ring
 //   warps 0..7  two consumer warpgroups, 64 query rows each.  Per key block: S = Q.K_j^T (wgmma, both operands in shared
 //               memory, 32 fp32 scores per thread) -> bias: one table value for a block wholly beyond +-sat from
-//               the warp's rows, else an unclamped lookup in an edge-padded table; the key < T mask only in a ragged
+//               the warp's rows, else an unclamped lookup in an edge-padded table; the key < len mask only in a ragged
 //               last block -> online softmax in registers (exp2 domain; a row's four threads
 //               exchange maxima and sums by shuffles) -> P packed to bf16 in registers, which is exactly the A-operand
 //               fragment of the next wgmma -> O += P.V_j (wgmma with A from registers, B = V^T_j in shared memory).
@@ -48,6 +48,7 @@ constexpr int SMEM = BAR_KV_EMPTY + 8 * KV_STAGES + 1024;  // + slack for aligni
 struct Args {
   __nv_bfloat16* out;
   const float* rel;
+  const int32_t* frames;  // (B) key length of every batch row, null: every row has T
   int sat, B, T, H, d;
 };
 
@@ -62,7 +63,10 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   const int q0 = blockIdx.x * AQ;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
-  const int nblk = (a.T + AK - 1) / AK;
+  // this batch row's own length: keys, queries and stores stop there (rows of a shorter call in a longer launch)
+  const int len = a.frames != nullptr ? __ldg(a.frames + b) : a.T;
+  if (q0 >= len) return;  // the whole CTA, before any barrier or TMA work
+  const int nblk = (len + AK - 1) / AK;
   const int sat = a.sat;
 
   if (warp == 8 && lane == 0) {
@@ -109,7 +113,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   const int kc = 2 * (lane & 3);                                 // first key column of this thread inside an n8 block
   const uint32_t sQ = sb + OFF_Q + wg * (64 * 128);
   const float c = 0.125f * LOG2E;                                // 1/sqrt(64) folded with log2(e)
-  const bool ragged = (a.T % AK) != 0;
+  const bool ragged = (len % AK) != 0;
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -144,7 +148,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             int rel = key - (qr + 8 * r);
             rel = rel < -sat ? -sat : (rel > sat ? sat : rel);
             float t = __fmaf_rn(s[4 * i + 2 * r + e], c, lds_f32(sb + OFF_BIAS + 4u * (rel + sat + PAD)));
-            if (key >= a.T) t = -INFINITY;
+            if (key >= len) t = -INFINITY;
             s[4 * i + 2 * r + e] = t;
           }
         }
@@ -174,7 +178,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     for (int r = 0; r < 2; ++r) {
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m[r], mx[r]);      // finite: every block has a key < T
+      const float m_new = fmaxf(m[r], mx[r]);      // finite: every block has a key < len
       alpha[r] = fast_exp2(m[r] - m_new);          // 0 on the first block
       m[r] = m_new;
       l[r] *= alpha[r];
@@ -218,7 +222,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int q = qr + 8 * r;
-    if (q < a.T) {
+    if (q < len) {
       const float inv_l = 1.0f / l[r];
       uint32_t* orow = reinterpret_cast<uint32_t*>(a.out + (static_cast<size_t>(b) * a.T + q) * a.d + h * DH + kc);
 #pragma unroll
@@ -241,6 +245,7 @@ cudaError_t launch_attention(const AttnPlan& p, cudaStream_t st) {
   att::Args a;
   a.out = reinterpret_cast<__nv_bfloat16*>(p.out);
   a.rel = p.rel;
+  a.frames = p.frames;
   a.sat = p.sat; a.B = p.B; a.T = p.T; a.H = p.H; a.d = p.H * att::DH;
   dim3 grid((p.T + att::AQ - 1) / att::AQ, p.H, p.B);
   att::attention_wgmma_kernel<<<grid, att::THREADS, att::SMEM, st>>>(p.tmQ, p.tmK, p.tmVT, a);

@@ -72,6 +72,7 @@ struct GemmArgs {
   int C, ncc, V, mask_token;
   // ---- adapted variants (ADAPT): per-row LoRA update of the accumulators, see lora_update() ----
   AdapterRefs lora;
+  const int32_t* frames;    // EPI_QKV: (B) frames of every batch row, null = T; v^T columns t >= frames[b] get 0
 };
 
 __device__ __forceinline__ float gelu_tanh(float x) {
@@ -552,9 +553,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const int d = g.N - g.d2;
                 __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(g.out2) +
                                    (static_cast<size_t>(b_idx) * d + (col0 - g.d2)) * g.Tpad + t_idx;
+                // a frame past its call's own length is a zero key column, as in the call's own launch (zeroed
+                // padding, TMA out-of-bounds fill); a select, so whatever the padded row holds cannot leak in
+                const bool pad = g.frames != nullptr && t_idx >= __ldg(g.frames + b_idx);
 #pragma unroll
                 for (int j = 0; j < 32; ++j)
-                  o[static_cast<size_t>(j) * g.Tpad] = __float2bfloat16_rn(__uint_as_float(v[j]) * rs);
+                  o[static_cast<size_t>(j) * g.Tpad] =
+                      pad ? __float2bfloat16_rn(0.f) : __float2bfloat16_rn(__uint_as_float(v[j]) * rs);
               }
               continue;
             }
@@ -811,6 +816,7 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
   g.zcur = p.zcur; g.dyn = p.dyn; g.rowgrp = p.rowgrp; g.partials = reinterpret_cast<float4*>(p.partials);
   g.C = p.C; g.ncc = p.ncc; g.V = p.V; g.mask_token = p.mask_token;
   g.lora = p.lora;
+  g.frames = p.epi == VNB_EPI_QKV ? p.frames : nullptr;
   if (p.lora.table != nullptr) {
     if (!p.lora.grp_adapter || !p.lora.rowgrp || !p.lora.u || p.lora.rows_per_grp < 1) return cudaErrorInvalidValue;
     switch (p.epi) {

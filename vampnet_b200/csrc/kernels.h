@@ -93,6 +93,9 @@ struct GemmPlan {
   int C = 0, ncc = 0, V = 0, mask_token = 0;
   // adapted variant of QKV / RESID / GEGLU (null table: the plain kernel): acc += u[row] . B'[col] for adapted rows
   AdapterRefs lora;
+  // VNB_EPI_QKV of a launch whose calls have different lengths: (B) frames of every batch row; v^T column t of batch row
+  // b is written as 0 for t >= frames[b] (null: every row has T frames)
+  const int32_t* frames = nullptr;
 };
 // Fills the tensor maps; A (M,K) bf16, W (N,K) bf16.
 bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out, void* out2,
@@ -112,6 +115,7 @@ struct AttnPlan {
   CUtensorMap tmVT;  // (B, d, Tpad) box (1, 64 rows, 64 cols)
   void* out = nullptr;         // (B, T, d) bf16
   const float* rel = nullptr;  // (2*sat+1, H)
+  const int32_t* frames = nullptr;  // (B) key length of every batch row (device); null: every row has T
   int sat = 0, B = 0, T = 0, Tpad = 0, H = 0;
 };
 bool make_attn_plan(AttnPlan* p, const void* qk, const void* vT, void* out, const float* rel, int sat, int B, int T,

@@ -348,7 +348,7 @@ class Interface(torch.nn.Module):
         return self._vamp_result(z, zv, coarse_start, fine_start, return_mask)
 
     @torch.inference_mode()
-    def vamp_many(self, requests: list):
+    def vamp_many(self, requests: list, mixed_lengths: bool = False):
         """Serve many vamp() calls together.  Each request is a dict of vamp() arguments (codes, mask, and optionally
         batch_size, feedback_steps, time_stretch_factor, return_mask and generate keyword arguments).  Returns the
         list the sequential vamp() calls return, bit for bit, and leaves the random, numpy and torch RNG states as
@@ -356,8 +356,12 @@ class Interface(torch.nn.Module):
 
         The requests advance stage by stage: feedback pass i runs the chunks of every request that has a pass i as
         one generate_many(), then the fine stage runs every request's chunks as one more.  Chunks of equal length,
-        within a request or across requests, so share launches."""
+        within a request or across requests, so share launches.
+
+        mixed_lengths=True: chunks of different lengths share launches too (generate_many(mixed_lengths=True) in both
+        stages), so a request's remainder chunk need not run in a launch of its own; the results are the same."""
         from .modules.transformer import draw_philox_key
+        many = dict(mixed_lengths=True) if mixed_lengths else {}
         reqs = []
         for r in requests:
             r = dict(r)
@@ -384,14 +388,14 @@ class Interface(torch.nn.Module):
             plans = [self._coarse_plan(q["zv"], q["mask"]) for q in stage]
             calls = [dict(**c, return_signal=False, philox_key=k, **q["gen"])
                      for q, plan in zip(stage, plans) for c, k in zip(plan, q["keys"][i])]
-            results = iter(self.coarse.generate_many(self.codec, calls))
+            results = iter(self.coarse.generate_many(self.codec, calls, **many))
             for q, plan in zip(stage, plans):
                 q["zv"], start = self._coarse_stitch(q["zv"], plan, [next(results) for _ in plan], True)
                 q["coarse_start"] = start.roll(shifts=(i + 1) % q["feedback_steps"], dims=-1)
         plans = [self._c2f_plan(self._with_fine_books(q["z"], q["zv"]), q["mask"]) for q in reqs]
         calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **self._C2F_KWARGS, **q["with_adapter"])
                  for q, (chunks, _) in zip(reqs, plans) for c, k in zip(chunks, q["c2f_keys"])]
-        results = iter(self.c2f.generate_many(self.codec, calls))
+        results = iter(self.c2f.generate_many(self.codec, calls, **many))
         out = []
         for q, (chunks, state) in zip(reqs, plans):
             zv, fine_start = self._c2f_stitch([next(results) for _ in chunks], state, True)

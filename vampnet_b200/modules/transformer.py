@@ -671,7 +671,7 @@ class VampNet(nn.Module):
         return out
 
     @torch.inference_mode()
-    def generate_many(self, codec, calls):
+    def generate_many(self, codec, calls, mixed_lengths: bool = False):
         """Run many independent generate() calls, batched into as few launches as the shapes allow.
 
         `calls` is a list of dicts of generate() keyword arguments.  The result equals
@@ -679,7 +679,11 @@ class VampNet(nn.Module):
         global RNG states afterwards are those the sequential calls leave: keys are drawn (draw_philox_key) in list
         order.  Calls with the same T, sampling steps and top-p on/off share one vnb_generate_many launch, in which
         each keeps its own N0, temperatures, schedules, top_p, key and adapter; a launch whose B*T would exceed
-        MANY_MAX_ROWS is split."""
+        MANY_MAX_ROWS is split.
+
+        mixed_lengths=True: calls of different T share launches too (one vnb_generate_ragged per (steps, top-p on/off)
+        bucket and MANY_MAX_ROWS).  Each call is padded to its launch's longest T with kept frames (code 0, mask 0)
+        that attention does not read, and its result is cut back to its own T; the results are still bit-identical."""
         import inspect
         sig = inspect.signature(VampNet.generate)
         prepared, want_signal = [], []
@@ -692,7 +696,7 @@ class VampNet(nn.Module):
                                                a["ctrl_masks"], a["top_p"], a["seed"], a["sample_cutoff"],
                                                a["cfg_guidance"], a["philox_key"], a["adapter"]))
             want_signal.append(bool(a["return_signal"]))
-        outs = self._launch_calls(prepared)
+        outs = self._launch_calls(prepared, mixed_lengths)
         return [self.decode(o, codec) if sig_ else o for o, sig_ in zip(outs, want_signal)]
 
     def _prepare_call(self, codec, time_steps, steps, start_tokens, temperature, mask, mask_temperature, ctrls,
@@ -732,21 +736,28 @@ class VampNet(nn.Module):
                     do_sample=[1 if (i / steps) <= sample_cutoff else 0 for i in range(steps)], key=k,
                     top_p=float(top_p) if (top_p is not None and top_p < 1.0) else 0.0, adapter=adapter)
 
-    def _launch_calls(self, calls: list) -> list:
+    def _launch_calls(self, calls: list, mixed_lengths: bool = False) -> list:
         """Launch prepared calls, one vnb_generate_many per (T, steps, top-p on) bucket of at most MANY_MAX_ROWS rows
-        (a single larger call runs alone); returns each call's (B, C, T) int64 tokens in list order."""
+        (a single larger call runs alone); returns each call's (B, C, T) int64 tokens in list order.
+        mixed_lengths: buckets are (steps, top-p on) only; a bucket's calls, longest first, fill launches while
+        rows * (the launch's longest T) stays within MANY_MAX_ROWS."""
         buckets = {}
         for i, c in enumerate(calls):
             top_p_on = 0.0 < c["top_p"] < 1.0
-            buckets.setdefault((c["z"].shape[-1], c["steps"], top_p_on), []).append(i)
+            T = None if mixed_lengths else c["z"].shape[-1]
+            buckets.setdefault((T, c["steps"], top_p_on), []).append(i)
         launches = []
-        for (T, _, _), idx in buckets.items():
-            cur, rows = [], 0
+        for idx in buckets.values():
+            if mixed_lengths:  # stable: calls of equal T keep their list order
+                idx = sorted(idx, key=lambda i: -calls[i]["z"].shape[-1])
+            cur, rows, T = [], 0, 0
             for i in idx:
                 B = calls[i]["z"].shape[0]
                 if cur and (rows + B) * T > MANY_MAX_ROWS:
                     launches.append(cur)
                     cur, rows = [], 0
+                if not cur:
+                    T = calls[i]["z"].shape[-1]  # the launch's T: its first (longest) call's
                 cur.append(i)
                 rows += B
             launches.append(cur)
@@ -754,7 +765,8 @@ class VampNet(nn.Module):
         keep = []
         for idx in launches:
             group = [calls[i] for i in idx]
-            for i, o in zip(idx, self._launch_group(group, keep)):
+            launch = self._launch_ragged if mixed_lengths else self._launch_group
+            for i, o in zip(idx, launch(group, keep)):
                 outs[i] = o
         # graph replay bakes the input pointers: keep them alive until the stream has consumed them
         self._last_io = keep
@@ -773,6 +785,30 @@ class VampNet(nn.Module):
                 default = (torch.arange(self.n_codebooks, device=dev) >= self.n_conditioning_codebooks).to(torch.int32)
                 m32 = torch.cat([c["mask"] if c["mask"] is not None else default[None, :, None].expand_as(c["z"])
                                  for c in calls]).contiguous()
+        out = self._launch(calls, keep, z, m32)
+        return list(out.split([c["z"].shape[0] for c in calls]))
+
+    def _launch_ragged(self, calls: list, keep: list) -> list:
+        """One vnb_generate_ragged launch of calls whose T may differ: each call's z and mask are padded to the longest
+        T with kept frames (code 0, mask 0), every call gets a materialised mask (the default one where it has none:
+        predicted codebooks masked, transformer.py:749-751), and each result is cut back to the call's own T."""
+        T = max(c["z"].shape[-1] for c in calls)
+        default = (torch.arange(self.n_codebooks, device=self.device) >= self.n_conditioning_codebooks).to(torch.int32)
+        zs, ms = [], []
+        for c in calls:
+            m = c["mask"] if c["mask"] is not None else default[None, :, None].expand_as(c["z"])
+            pad = (0, T - c["z"].shape[-1])
+            zs.append(torch.nn.functional.pad(c["z"], pad, value=0))
+            ms.append(torch.nn.functional.pad(m, pad, value=0))
+        out = self._launch(calls, keep, torch.cat(zs).contiguous(), torch.cat(ms).contiguous(),
+                           frames=[c["z"].shape[-1] for c in calls])
+        parts = out.split([c["z"].shape[0] for c in calls])
+        return [o if c["z"].shape[-1] == T else o[..., :c["z"].shape[-1]].contiguous() for o, c in zip(parts, calls)]
+
+    def _launch(self, calls: list, keep: list, z, m32, frames=None):
+        """One launch of the prepared calls on their concatenated (B, C, T) z / mask; frames: each call's own length
+        (vnb_generate_ragged), None when all have T."""
+        dev = self.device
         B, _, T = z.shape
         steps = calls[0]["steps"]
         arrays = []
@@ -785,18 +821,23 @@ class VampNet(nn.Module):
             g.seed_lo, g.seed_hi, g.top_p = c["key"] & 0xFFFFFFFF, (c["key"] >> 32) & 0xFFFFFFFF, c["top_p"]
         gam = (C.c_float * steps)(*calls[0]["gamma"])
         ids = [self._adapter_id(c.get("adapter")) for c in calls]
+        ids = (C.c_int32 * len(calls))(*ids) if any(i >= 0 for i in ids) else None
         out = torch.empty_like(z)
         graph = 1 if self.use_cuda_graph else 0
         with torch.cuda.device(dev):
-            if any(i >= 0 for i in ids):
+            if frames is not None:
+                _lib.check(_lib.lib().vnb_generate_ragged(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam,
+                                                          groups, len(calls), (C.c_int32 * len(calls))(*frames), ids,
+                                                          graph, _lib.ptr(out), _lib.stream_ptr(dev)))
+            elif ids is not None:
                 _lib.check(_lib.lib().vnb_generate_many_adapted(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps,
-                                                                gam, groups, len(calls), (C.c_int32 * len(calls))(*ids),
-                                                                graph, _lib.ptr(out), _lib.stream_ptr(dev)))
+                                                                gam, groups, len(calls), ids, graph, _lib.ptr(out),
+                                                                _lib.stream_ptr(dev)))
             else:  # no call has an adapter: the plain kernels and graph
                 _lib.check(_lib.lib().vnb_generate_many(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam,
                                                         groups, len(calls), graph, _lib.ptr(out), _lib.stream_ptr(dev)))
         keep.append((z, m32, out))
-        return list(out.split([c["z"].shape[0] for c in calls]))
+        return out
 
     @torch.no_grad()
     def decode(self, z, codec):
