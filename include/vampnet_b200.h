@@ -184,6 +184,25 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
                             const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
                             const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
                             void* stream);
+/* vnb_generate_ragged for calls of different sampling-step counts: group g runs group_steps[g] steps (host [n_groups],
+ * each in 1..256, in NON-INCREASING order) with its own gamma schedule group_gamma[g] (host, [group_steps[g]]); its
+ * temp_eff and do_sample have group_steps[g] entries.  The launch runs S = group_steps[0] iterations.  Group g is idle
+ * for the first S - group_steps[g] of them: its state is not touched and no kernel does work for its rows.  From then
+ * on, iteration i is its own step j = i - (S - group_steps[g]), with gamma[j], temp_eff[j], do_sample[j], Philox step
+ * word j and the last-step flag on j = group_steps[g] - 1, so every group ends on the launch's last iteration.  Each
+ * group's out therefore equals, bit for bit, vnb_generate_ragged of its rows alone with its own steps.  Because of the
+ * order, the rows live at an iteration are a prefix of the batch: the GEMMs, attention, the embedding, the LoRA
+ * down-projections and the sampler skip the tiles, CTAs and rows wholly past it, so an idle iteration costs close to
+ * nothing.  group_frames and group_adapter may be NULL as in vnb_generate_ragged.  Every group with the same count:
+ * vnb_generate_ragged's kernels and graph (each group still uses its own gamma).  Otherwise the launch runs the
+ * live-bounded kernels (one more graph per workspace key); the per-iteration live-row table is written before every
+ * launch or replay, so one (B, T, S) graph serves any assignment of step counts <= S and any grouping.
+ * Errors: those of vnb_generate_ragged, NULL group_steps, group_gamma or group_gamma[g], a count outside 1..256 and
+ * counts that increase from one group to the next. */
+int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                           const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
+                           int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
+                           int32_t use_graph, int64_t* out, void* stream);
 /* One sampling iteration on caller-supplied logits (B, S, V) fp32 — sample_from_logits +
  * mask_by_random_topk + the where()s around them (transformer.py:849-932).  State is explicit:
  * zflat (B, S) int32 in "t c" order (util.py:39) is updated in place; tokens_out (B, S) int32
@@ -199,8 +218,9 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
  * number of kernel nodes it contains).
  * vnb_graph_capture_count: generate graphs captured so far (a weight hot swap or a repeated call must not
  * add to it: graphs are cached per (workspace, steps, mask, top_p, adapted or not, some group shorter than T or
- * not); the grouping of vnb_generate_many, the group -> adapter table and the per-row frames of vnb_generate_ragged
- * are not part of that key).
+ * not, some group with fewer steps than the launch or not); the grouping of vnb_generate_many, the group -> adapter
+ * table, the per-row frames of vnb_generate_ragged and the step counts of vnb_generate_steps are not part of that
+ * key).
  * vnb_profile_begin/end: between the two calls every launch of forward/generate is bracketed by CUDA
  * events on the launching stream (graph replay is bypassed so that the events can be recorded);
  * end() returns the summed device time and launch count per kernel family:
@@ -250,6 +270,13 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
  * frames[b] do no work. */
 int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                                  int32_t B, int32_t T, int32_t Tpad, int32_t H, const int32_t* frames, void* stream);
+/* Test-only: the live bound that the unit-level entry points of this calling thread (vnb_op_gemm, vnb_op_attention and
+ * every vnb_dbg_* op) give their kernels from now on, as vnb_generate_steps gives it at every iteration.  live: DEVICE
+ * pointer to one int32 R, or NULL (the default: every row is live).  Batch rows b >= R are idle: GEMM tiles whose
+ * first row is at or past R * T (pair: the cluster's first row) and attention CTAs of rows b >= R do no work, the
+ * LoRA down-projection and the sampler (vnb_dbg_sample) leave those rows untouched.  Live rows are bit-equal to a
+ * launch without a bound; dead rows of a tile that straddles R * T are unspecified. */
+int32_t vnb_dbg_set_live(const int32_t* live);
 /* Naive SIMT GEMM used only to bisect the tensor-core path in tests: out fp32 (M, N) = A x W^T. */
 int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int32_t K, float* out, void* stream);
 /* Test-only: vnb_op_gemm plus the fused-RMSNorm plumbing the forward uses, epi in {BF16, QKV, RESID, GEGLU, BIAS_F32}.

@@ -1,7 +1,7 @@
 """Throughput of an app-shaped request mix: sequential Interface.vamp() calls against one Interface.vamp_many(), with and
 without mixed-length launches.
 
-    python tools/many_requests.py [--requests 16] [--repeats 3] [--out result.json]
+    python tools/many_requests.py [--requests 16] [--repeats 3] [--mixed-steps] [--out result.json]
 
 The app serves one vamp(batch_size=2) per request; a 10 s coarse chunk at B = 2 is M = 1150 GEMM rows, far below the
 batches the kernels are tuned at.  vamp_many runs every request's chunks stage by stage through generate_many, so
@@ -18,6 +18,12 @@ timed run ends in a device synchronise.  The outputs of the three arms are compa
 mismatch fails the run.  Per arm and timed run it also records the generate graphs captured
 (vnb_graph_capture_count), the generate launches, and the fraction of GEMM rows (batch rows x launch T) that are
 padding.  The card's name, power limit and maximum SM clock are read in the same run.
+
+--mixed-steps: every request draws its coarse sampling steps (seeded) from {12, 24, 36, 48, 64}, and the arms are the
+sequential loop, iface.vamp_many(requests, mixed_lengths=True) and iface.vamp_many(requests, mixed_lengths=True,
+mixed_steps=True).  The run also records the device time per kernel family of one profiled run of each vamp_many arm
+(vnb_profile_begin / end; graphs are bypassed while profiling), and times one coarse launch of two B = 2, T = 575 calls
+of 48 and 12 steps (generate_many(mixed_steps=True)) against the two calls launched one by one.
 """
 from __future__ import annotations
 
@@ -64,7 +70,10 @@ def build_iface():
     return Interface.from_models(codec, models[0], models[1], device="cuda")
 
 
-def make_requests(iface, n, seed):
+STEP_CHOICES = (12, 24, 36, 48, 64)
+
+
+def make_requests(iface, n, seed, mixed_steps=False):
     g = torch.Generator().manual_seed(seed)
     reqs = []
     for _ in range(n):
@@ -74,7 +83,10 @@ def make_requests(iface, n, seed):
         mask = torch.ones_like(z)
         mask[:, :, ::7] = 0          # periodic prompt
         mask[:, 3:, :] = 1           # codebooks >= 3 always regenerated
-        reqs.append(dict(codes=z.cuda(), mask=mask.cuda(), batch_size=2, _sampling_steps=36, return_mask=False))
+        steps = 36
+        if mixed_steps:
+            steps = STEP_CHOICES[int(torch.randint(0, len(STEP_CHOICES), (1,), generator=g))]
+        reqs.append(dict(codes=z.cuda(), mask=mask.cuda(), batch_size=2, _sampling_steps=steps, return_mask=False))
     return reqs
 
 
@@ -87,7 +99,8 @@ def reseed(s):
 class LaunchTally:
     """Counts the generate launches made through vampnet_b200._lib while installed, with their GEMM rows (B x T) and
     how many of those rows are padding (vnb_generate_ragged: rows of a call past its own frames)."""
-    NAMES = ("vnb_generate", "vnb_generate_many", "vnb_generate_many_adapted", "vnb_generate_ragged")
+    NAMES = ("vnb_generate", "vnb_generate_many", "vnb_generate_many_adapted", "vnb_generate_ragged",
+             "vnb_generate_steps")
 
     def __init__(self):
         from vampnet_b200 import _lib as L
@@ -107,7 +120,7 @@ class LaunchTally:
                     B, T = a[3], a[4]
                     tally.launches += 1
                     tally.rows += B * T
-                    if name == "vnb_generate_ragged" and a[9] is not None:
+                    if name in ("vnb_generate_ragged", "vnb_generate_steps") and a[9] is not None:
                         tally.pad_rows += sum(a[7][g].rows * (T - a[9][g]) for g in range(a[8]))
                     return fn(*a)
                 return counted
@@ -126,20 +139,75 @@ def timed(fn):
     return out, time.perf_counter() - t0
 
 
+def family_times(iface, fn):
+    """Device ms and launches per kernel family, summed over both models, of one profiled run of fn."""
+    import ctypes as C
+    from vampnet_b200 import _lib as L
+    n = len(L.FAMILIES) + 1
+    handles = [iface.coarse._handle, iface.c2f._handle]
+    for h in handles:
+        L.check(L.lib().vnb_profile_begin(h))
+    fn()
+    torch.cuda.synchronize()
+    names = list(L.FAMILIES) + ["lora_down"]
+    ms, cnt = dict.fromkeys(names, 0.0), dict.fromkeys(names, 0)
+    for h in handles:
+        t, k = (C.c_float * n)(), (C.c_int32 * n)()
+        L.check(L.lib().vnb_profile_end(h, t, k, n))
+        for i, name in enumerate(names):
+            ms[name] += t[i]
+            cnt[name] += k[i]
+    return {k: round(v, 2) for k, v in ms.items() if cnt[k]}, {k: v for k, v in cnt.items() if v}
+
+
+def pair_launch(iface, repeats=5):
+    """One coarse launch of a 48-step and a 12-step call (B = 2, T = 575 each) against the two launched alone."""
+    g = torch.Generator().manual_seed(5)
+    model, codec = iface.coarse, iface.codec
+
+    def call(steps, seed):
+        z = torch.randint(0, 1024, (2, 4, 575), generator=g).cuda()
+        mask = (torch.rand(2, 4, 575, generator=g) < 0.7).long().cuda()
+        return dict(start_tokens=z, mask=mask, _sampling_steps=steps, seed=seed, return_signal=False)
+    c48, c12 = call(48, 1), call(12, 2)
+    arms = {"mixed_48_12": lambda: model.generate_many(codec, [c48, c12], mixed_steps=True),
+            "alone_48": lambda: [model.generate(codec, **c48)], "alone_12": lambda: [model.generate(codec, **c12)]}
+    times, outs = {}, {}
+    for name, fn in arms.items():
+        fn()
+        ts = []
+        for _ in range(repeats):
+            o, dt = timed(fn)
+            ts.append(dt)
+        outs[name], times[name] = o, ts
+    med = {k: round(float(np.median(v)) * 1e3, 2) for k, v in times.items()}
+    return {"ms": {k: [round(t * 1e3, 2) for t in v] for k, v in times.items()}, "median_ms": med,
+            "separate_sum_ms": round(med["alone_48"] + med["alone_12"], 2),
+            "extra_over_alone_48_ms": round(med["mixed_48_12"] - med["alone_48"], 2),
+            "bit_identical": bool(torch.equal(outs["mixed_48_12"][0], outs["alone_48"][0]) and
+                                  torch.equal(outs["mixed_48_12"][1], outs["alone_12"][0]))}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=16)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--mixed-steps", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     iface = build_iface()
-    reqs = make_requests(iface, a.requests, a.seed)
+    reqs = make_requests(iface, a.requests, a.seed, a.mixed_steps)
     frames = [r["codes"].shape[-1] for r in reqs]
     from vampnet_b200 import _lib as L
-    runs = {"sequential": lambda: [iface.vamp(**r) for r in reqs], "vamp_many": lambda: iface.vamp_many(reqs),
-            "vamp_many_mixed": lambda: iface.vamp_many(reqs, mixed_lengths=True)}
+    if a.mixed_steps:
+        runs = {"sequential": lambda: [iface.vamp(**r) for r in reqs],
+                "vamp_many_mixed": lambda: iface.vamp_many(reqs, mixed_lengths=True),
+                "vamp_many_mixed_steps": lambda: iface.vamp_many(reqs, mixed_lengths=True, mixed_steps=True)}
+    else:
+        runs = {"sequential": lambda: [iface.vamp(**r) for r in reqs], "vamp_many": lambda: iface.vamp_many(reqs),
+                "vamp_many_mixed": lambda: iface.vamp_many(reqs, mixed_lengths=True)}
     names = list(runs)
     warm_captures = {}
     for name, fn in runs.items():  # warm-up: workspaces, graph captures
@@ -164,15 +232,14 @@ def main():
         for name in names[1:]:
             identical &= all(torch.equal(x, y) for x, y in zip(outs["sequential"], outs[name]))
     tokens = 2 * sum(frames)  # batch_size 2 per request
+    med = {k: float(np.median(v)) for k, v in times.items()}
     res = {
         "card": card(),
-        "requests": a.requests, "frames": frames, "batch_size": 2, "coarse_steps": 36, "c2f_steps": 2,
+        "requests": a.requests, "frames": frames, "batch_size": 2,
+        "coarse_steps": [r["_sampling_steps"] for r in reqs] if a.mixed_steps else 36, "c2f_steps": 2,
         "seconds": {k: [round(t, 4) for t in v] for k, v in times.items()},
-        "median_s": {k: round(float(np.median(v)), 4) for k, v in times.items()},
-        "tokens_per_s": {k: round(tokens / float(np.median(v)), 1) for k, v in times.items()},
-        "speedup_median": round(float(np.median(times["sequential"]) / np.median(times["vamp_many"])), 3),
-        "speedup_median_mixed": round(float(np.median(times["sequential"]) / np.median(times["vamp_many_mixed"])), 3),
-        "mixed_vs_vamp_many": round(float(np.median(times["vamp_many"]) / np.median(times["vamp_many_mixed"])), 3),
+        "median_s": {k: round(v, 4) for k, v in med.items()},
+        "tokens_per_s": {k: round(tokens / v, 1) for k, v in med.items()},
         "graph_captures_warmup": warm_captures,
         "graph_captures_timed": captures,
         "generate_launches": {k: t.launches for k, t in tallies.items()},
@@ -180,6 +247,20 @@ def main():
         "padding_row_fraction": {k: round(t.pad_rows / max(t.rows, 1), 4) for k, t in tallies.items()},
         "bit_identical": bool(identical),
     }
+    if a.mixed_steps:
+        res["speedup_median"] = {k: round(med["sequential"] / v, 3) for k, v in med.items() if k != "sequential"}
+        res["mixed_steps_vs_mixed"] = round(med["vamp_many_mixed"] / med["vamp_many_mixed_steps"], 3)
+        res["family_ms"], res["family_launches"] = {}, {}
+        for name in ("vamp_many_mixed", "vamp_many_mixed_steps"):
+            reseed(1)
+            res["family_ms"][name], res["family_launches"][name] = family_times(iface, runs[name])
+        res["pair_launch_48_12"] = pair_launch(iface)
+        identical &= res["pair_launch_48_12"]["bit_identical"]
+        res["bit_identical"] = bool(identical)
+    else:
+        res["speedup_median"] = round(med["sequential"] / med["vamp_many"], 3)
+        res["speedup_median_mixed"] = round(med["sequential"] / med["vamp_many_mixed"], 3)
+        res["mixed_vs_vamp_many"] = round(med["vamp_many"] / med["vamp_many_mixed"], 3)
     print(json.dumps(res))
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)

@@ -80,6 +80,9 @@ _SIGS = {
     "vnb_generate_ragged": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.POINTER(C.c_float), C.POINTER(GenGroup), C.c_int32, C.POINTER(C.c_int32),
                                         C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_generate_steps": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
+                                       C.POINTER(C.POINTER(C.c_float)), C.POINTER(GenGroup), C.c_int32,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_adapter_add": (C.c_int32, [C.c_void_p, C.POINTER(AdapterWeights), C.POINTER(C.c_int32)]),
     "vnb_adapter_remove": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vnb_forward_codes_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
@@ -108,6 +111,7 @@ _SIGS = {
     "vnb_codec_conv_in": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_void_p]),
     "vnb_codec_conv_out": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32] * 5 + [C.c_void_p]),
     "vnb_set_error_cuda": (C.c_int32, [C.c_char_p, C.c_int32]),
+    "vnb_dbg_set_live": (C.c_int32, [C.c_void_p]),
     "vnb_dbg_gemm_ref": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_dbg_gemm_fused": (C.c_int32, [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_float,

@@ -141,9 +141,10 @@ struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in w
   bool fused;   // sampler fused into the classifier epilogue (vnb_set_option "fused_sampler")
   bool adapted;  // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
   bool ragged;   // QKV and attention read the frames table (some group is shorter than T)
+  bool mixed_steps;  // every kernel of iteration i reads the live table (some group has fewer steps than the launch)
   bool operator<(const GraphKey& o) const {
-    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged) <
-           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged);
+    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged, mixed_steps) <
+           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged, o.mixed_steps);
   }
 };
 
@@ -160,6 +161,9 @@ struct Workspace {
   // launches of calls with different lengths: frames (B) = the length of every batch row's call, rewritten before every
   // launch or replay (read by the QKV epilogue and attention)
   DevBuf frames;
+  // launches of calls with different step counts: live (kMaxSteps) = the batch rows live at every iteration (a prefix),
+  // rewritten before every launch or replay (read by every kernel of the iteration)
+  DevBuf live;
   int embKp = 0;
   int ss_parts = 0;
   std::vector<GemmPlan> qkv, wo, up, down;
@@ -258,6 +262,7 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   CK(ws->rowgrp.alloc(sizeof(RowGroup) * B));
   CK(ws->grp_adapter.alloc(sizeof(int32_t) * B));
   CK(ws->frames.alloc(sizeof(int32_t) * B));
+  CK(ws->live.alloc(sizeof(int32_t) * vnb_model::kMaxSteps));
   CK(ws->lora_u.alloc(M * 16 * 4));
   CK(ws->z_in.alloc(M * c.n_codebooks * 8));
   CK(ws->mask_in.alloc(M * c.n_codebooks * 4));
@@ -325,12 +330,16 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   } while (0)
 
 // CodebookEmbedding (layers.py:134-162): gather (+ split) the latents, then the out_proj contraction on the tensor cores.
-static int run_embed(vnb_model* m, Workspace* ws, const int32_t* codes_btc, const float* latents, cudaStream_t st) {
+// live (device, null = every row): batch rows at or past live[0] are not embedded.
+static int run_embed(vnb_model* m, Workspace* ws, const int32_t* codes_btc, const float* latents, cudaStream_t st,
+                     const int32_t* live = nullptr) {
   const vnb_config& c = m->cfg;
   LAUNCH(FAM_EMBED, launch_embed_gather(codes_btc, latents, m->w.emb_table, ws->embA.p, ws->M, ws->T, c.n_codebooks,
                                         c.vocab_size + 1, c.n_codebooks * 8, ws->embKp, ws->ssA.as<float>(),
-                                        c.d_model / 256, ws->ss_parts, st));
-  LAUNCH(FAM_EMBED, launch_gemm(ws->emb, st));
+                                        c.d_model / 256, ws->ss_parts, live, st));
+  GemmPlan emb = ws->emb;
+  emb.live = live;
+  LAUNCH(FAM_EMBED, launch_gemm(emb, st));
   return 0;
 }
 
@@ -341,7 +350,7 @@ static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int 
     LAUNCH(fam, launch_gemm(plan, st));
     return 0;
   }
-  GemmPlan p = plan;
+  GemmPlan p = plan;  // carries the live bound of the iteration, which the down-projection shares
   p.lora.table = m->adapter_tab.as<AdapterDev>();
   p.lora.grp_adapter = ws->grp_adapter.as<int32_t>();
   p.lora.rowgrp = ws->rowgrp.as<RowGroup>();
@@ -349,15 +358,17 @@ static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int 
   p.lora.slot = slot;
   p.lora.layer = l;
   p.lora.u = ws->lora_u.as<float>();
-  LAUNCH(FAM_LORA_DOWN, launch_lora_down(a, p.M, p.K, p.lora, st));
+  LAUNCH(FAM_LORA_DOWN, launch_lora_down(a, p.M, p.K, p.lora, p.live, p.T, st));
   LAUNCH(fam, launch_gemm(p, st));
   return 0;
 }
 
 // x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  ragged: batch row b
-// is a call of ws->frames[b] frames; its later frames are padding that no earlier frame attends to.
+// is a call of ws->frames[b] frames; its later frames are padding that no earlier frame attends to.  live (device, null
+// = every row): batch rows at or past live[0] are idle; every kernel skips the tiles and CTAs wholly past them.
 static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st, float* acts = nullptr,
-                     const SampleDyn* fused_dyn = nullptr, bool adapted = false, bool ragged = false) {
+                     const SampleDyn* fused_dyn = nullptr, bool adapted = false, bool ragged = false,
+                     const int32_t* live = nullptr) {
   const vnb_config& c = m->cfg;
   // RMSNorm (transformer.py:43-58) is fused: norm weights are folded into wqkv / w1 / wcls at pack time, the
   // producers of x (embed, attn-out, ffn-down) also emit bf16(x) and per-row sums of squares, and the consumers
@@ -365,24 +376,30 @@ static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st
   const int32_t* frames = ragged ? ws->frames.as<int32_t>() : nullptr;
   AttnPlan attn = ws->attn;
   attn.frames = frames;
+  attn.live = live;
+  const auto bounded = [live](const GemmPlan& p) {
+    GemmPlan q = p;
+    q.live = live;
+    return q;
+  };
   for (int l = 0; l < c.n_layers; ++l) {
-    GemmPlan qkv = ws->qkv[l];
+    GemmPlan qkv = bounded(ws->qkv[l]);
     qkv.frames = frames;
     if (run_lora_gemm(m, ws, qkv, FAM_GEMM_QKV, adapted, LORA_QKV, l, ws->y.p, st)) return 1;
     LAUNCH(FAM_ATTN, launch_attention(attn, st));
-    if (run_lora_gemm(m, ws, ws->wo[l], FAM_GEMM_O, adapted, LORA_WO, l, ws->att.p, st) ||
-        run_lora_gemm(m, ws, ws->up[l], FAM_GEMM_UP, adapted, LORA_W1, l, ws->y.p, st) ||
-        run_lora_gemm(m, ws, ws->down[l], FAM_GEMM_DOWN, adapted, LORA_W2, l, ws->h.p, st))
+    if (run_lora_gemm(m, ws, bounded(ws->wo[l]), FAM_GEMM_O, adapted, LORA_WO, l, ws->att.p, st) ||
+        run_lora_gemm(m, ws, bounded(ws->up[l]), FAM_GEMM_UP, adapted, LORA_W1, l, ws->y.p, st) ||
+        run_lora_gemm(m, ws, bounded(ws->down[l]), FAM_GEMM_DOWN, adapted, LORA_W2, l, ws->h.p, st))
       return 1;
     if (acts)  // return_activations: the residual stream after this layer (transformer.py:455-456)
       CK(cudaMemcpyAsync(acts + static_cast<size_t>(l) * ws->M * c.d_model, ws->x.p, ws->x.n, cudaMemcpyDeviceToDevice, st));
   }
   if (fused_dyn != nullptr) {  // generate loop: sample in the classifier's epilogue, no logits tensor
-    GemmPlan cls = ws->cls_sample;
+    GemmPlan cls = bounded(ws->cls_sample);
     cls.dyn = fused_dyn;
     LAUNCH(FAM_GEMM_CLS, launch_gemm(cls, st));
   } else {
-    GemmPlan cls = ws->cls;
+    GemmPlan cls = bounded(ws->cls);
     cls.out = logits;
     LAUNCH(FAM_GEMM_CLS, launch_gemm(cls, st));
   }
@@ -582,8 +599,9 @@ static int fused_sampler_enabled() {
   return g_fused_sampler;
 }
 
+// mixed_steps: iteration i runs only the batch rows ws->live[i] counts (a prefix); the others are idle and untouched.
 static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int steps, int64_t* out,
-                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged) {
+                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged, bool mixed_steps) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
   // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
@@ -599,13 +617,15 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   sa.rowgrp = ws->rowgrp.as<RowGroup>();
   sa.B = ws->B; sa.T = ws->T; sa.C = c.n_codebooks; sa.ncc = ncc; sa.V = c.vocab_size; sa.mask_token = c.vocab_size;
   for (int i = 0; i < steps; ++i) {
-    if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
+    const int32_t* live = mixed_steps ? ws->live.as<int32_t>() + i : nullptr;
+    sa.live = live;
+    if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st, live)) return 1;
     const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
     if (fused) {
-      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted, ragged)) return 1;
+      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted, ragged, live)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
     } else {
-      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted, ragged)) return 1;
+      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted, ragged, live)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_step_dev(sa, dyn_i, st, use_top_p));
     }
     ++g_launches;  // sample step = two kernels
@@ -615,13 +635,18 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   return 0;
 }
 
-int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
-                            const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
-                            const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
-                            void* stream) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+}  // extern "C"
+
+// The launch behind vnb_generate_ragged and vnb_generate_steps: group g runs group_steps[g] steps (NULL: every group
+// runs `steps`) with its own gamma schedule group_gamma[g] (NULL: every group uses `gamma`).  The caller has checked the
+// steps and their order; `steps` is their maximum S.  Group g is idle for the first S - steps_g iterations and then runs
+// its own step j = i - (S - steps_g) with j's schedule values, Philox step word and last-step flag.
+static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                           const float* gamma, const int32_t* group_steps, const float* const* group_gamma,
+                           const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
+                           const int32_t* group_adapter, int32_t use_graph, int64_t* out, cudaStream_t st) {
   if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
-  if (!gamma || !groups) return fail("vnb_generate_many: gamma and groups are required");
+  if ((!gamma && !group_gamma) || !groups) return fail("vnb_generate_many: gamma and groups are required");
   if (B < 1 || T < 1) return fail("vnb_generate_many: need B >= 1 and T >= 1 (got %d, %d)", B, T);
   if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
   const auto top_p_on = [](float tp) { return tp > 0.f && tp < 1.f; };
@@ -647,28 +672,38 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
   if (ragged && !mask) return fail("vnb_generate_ragged: a launch with groups shorter than T needs a mask");
   if (check_adapter_ids(m, group_adapter, n_groups, "vnb_generate_many_adapted")) return 1;
   const bool adapted = any_adapted(group_adapter, n_groups);
+  bool mixed_steps = false;
+  for (int g = 0; group_steps && g < n_groups; ++g) mixed_steps |= group_steps[g] != steps;
   Workspace* ws;
   if (get_workspace(m, B, T, &ws)) return 1;
   m->last = ws;
-  // the [step][group] table (row stride B) and the row map, pageable sources: the runtime stages them before
-  // returning, so the vectors may die at scope exit
+  // the [step][group] table (row stride B), the row map and the live rows per iteration, pageable sources: the runtime
+  // stages them before returning, so the vectors may die at scope exit
   std::vector<SampleDyn> dyn(static_cast<size_t>(steps) * B);
   std::vector<RowGroup> rowgrp(B);
   std::vector<int32_t> frames(ragged ? B : 0);
+  std::vector<int32_t> live(mixed_steps ? steps : 0, 0);
   for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
     const vnb_gen_group& q = groups[g];
     const float inv_t = inv_temperature(q.temperature);
+    const int steps_g = group_steps ? group_steps[g] : steps;
+    const float* gam = group_gamma ? group_gamma[g] : gamma;
+    const int idle = steps - steps_g;  // iterations before the group's first step
     for (int i = 0; i < steps; ++i) {
       SampleDyn& d = dyn[static_cast<size_t>(i) * B + g];
+      d = SampleDyn{};
       d.inv_temp = inv_t;
-      d.gamma = gamma[i];
-      d.temp_eff = q.temp_eff[i];
-      d.do_sample = q.do_sample[i];
-      d.is_last = (i == steps - 1);
-      d.step = i;
       d.seed_lo = q.seed_lo;
       d.seed_hi = q.seed_hi;
       d.top_p = q.top_p;
+      if (i < idle) continue;  // no kernel reads an idle group's entry
+      const int j = i - idle;
+      d.gamma = gam[j];
+      d.temp_eff = q.temp_eff[j];
+      d.do_sample = q.do_sample[j];
+      d.is_last = (j == steps_g - 1);
+      d.step = j;
+      if (mixed_steps) live[i] += q.rows;
     }
     for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
     for (int b = first; ragged && b < first + q.rows; ++b) frames[b] = group_frames[g];
@@ -676,11 +711,13 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
   CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * dyn.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
   if (ragged) CK(cudaMemcpyAsync(ws->frames.p, frames.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
+  if (mixed_steps) CK(cudaMemcpyAsync(ws->live.p, live.data(), sizeof(int32_t) * steps, cudaMemcpyHostToDevice, st));
   if (adapted && stage_adapters(m, ws, group_adapter, n_groups, st)) return 1;
   const bool fused = fused_sampler_enabled() != 0 && !use_top_p && ws->can_fuse;
   if (!fused && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
-  if (!use_graph || m->prof.on) return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged);
+  if (!use_graph || m->prof.on)
+    return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged, mixed_steps);
 
   const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
   CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
@@ -688,7 +725,7 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
   const int64_t* gz = ws->z_in.as<int64_t>();
   const int32_t* gmask = mask ? ws->mask_in.as<int32_t>() : nullptr;
   int64_t* gout = ws->z_out.as<int64_t>();
-  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged};
+  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged, mixed_steps};
   auto it = ws->graphs.find(key);
   if (it == ws->graphs.end()) {
     cudaStream_t cap;
@@ -697,7 +734,7 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cap); return fail("begin capture: %s", cudaGetErrorString(e)); }
     const unsigned long long before = g_launches;
-    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged);
+    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged, mixed_steps);
     const unsigned long long in_graph = g_launches - before;
     g_launches = before;
     e = cudaStreamEndCapture(cap, &graph);
@@ -721,6 +758,36 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
   g_launches += ws->graph_kernels[key];
   CK(cudaMemcpyAsync(out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+extern "C" {
+
+int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                            const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                            const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
+                            void* stream) {
+  return generate_launch(m, z, mask, B, T, steps, gamma, nullptr, nullptr, groups, n_groups, group_frames,
+                         group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                           const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
+                           int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
+                           int32_t use_graph, int64_t* out, void* stream) {
+  if (!group_steps || !group_gamma || !groups) return fail("vnb_generate_steps: group_steps, group_gamma and groups are required");
+  if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
+  for (int g = 0; g < n_groups; ++g) {
+    if (group_steps[g] < 1 || group_steps[g] > vnb_model::kMaxSteps)
+      return fail("vnb_generate_steps: group %d has %d sampling steps, outside 1..%d", g, group_steps[g],
+                  vnb_model::kMaxSteps);
+    // longest first: the live rows of every iteration are then a prefix of the batch
+    if (g > 0 && group_steps[g] > group_steps[g - 1])
+      return fail("vnb_generate_steps: group %d has %d steps, more than group %d's %d (the order must be non-increasing)",
+                  g, group_steps[g], g - 1, group_steps[g - 1]);
+    if (!group_gamma[g]) return fail("vnb_generate_steps: group %d lacks its schedules (gamma)", g);
+  }
+  return generate_launch(m, z, mask, B, T, group_steps[0], nullptr, group_steps, group_gamma, groups, n_groups,
+                         group_frames, group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // Calls of one length are the group_frames = NULL case.
@@ -821,11 +888,18 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
 }
 
 // ------------------------------------------------------------------------------- unit-level ops
+// vnb_dbg_set_live: the live bound the unit-level entry points below give their kernels (device, null = none)
+static thread_local const int32_t* g_dbg_live = nullptr;
+int32_t vnb_dbg_set_live(const int32_t* live) {
+  g_dbg_live = live;
+  return 0;
+}
 int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out, void* out2,
                     const float* bias, int32_t T, int32_t Tpad, void* stream) {
   GemmPlan p;
   const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
   if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
+  p.live = g_dbg_live;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -833,6 +907,7 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
                          int32_t T, int32_t Tpad, int32_t H, void* stream) {
   AttnPlan p;
   if (!make_attn_plan(&p, qk, vT, out, rel_bias, rel_sat, B, T, Tpad, H)) return fail("attn plan: %s", tmap_error());
+  p.live = g_dbg_live;
   CK(launch_attention(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -842,6 +917,7 @@ int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, cons
   AttnPlan p;
   if (!make_attn_plan(&p, qk, vT, out, rel_bias, rel_sat, B, T, Tpad, H)) return fail("attn plan: %s", tmap_error());
   p.frames = frames;
+  p.live = g_dbg_live;
   CK(launch_attention(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -867,6 +943,7 @@ int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M,
   if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
   p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
   if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
+  p.live = g_dbg_live;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -915,7 +992,8 @@ static int dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M
   p.lora.layer = layer;
   p.lora.u = u;
   p.frames = frames;
-  CK(launch_lora_down(A, M, K, p.lora, st));
+  p.live = g_dbg_live;
+  CK(launch_lora_down(A, M, K, p.lora, p.live, T, st));
   CK(launch_gemm(p, st));
   CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
   return 0;
@@ -946,6 +1024,7 @@ int32_t vnb_dbg_gemm_qkv_frames(const void* A, const void* W, int32_t M, int32_t
     return fail("gemm plan: %s", tmap_error());
   p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
   p.frames = frames;
+  p.live = g_dbg_live;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -968,6 +1047,7 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
   p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
   p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
   if (stage_sample_dyn(d, st, &p.dyn) || one_group_rows((M + T - 1) / T, &p.rowgrp)) return 1;
+  p.live = g_dbg_live;
   CK(launch_gemm(p, st));
   return 0;
 }
@@ -1014,6 +1094,7 @@ int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, 
   sa.logits = logits; sa.zcur = zcur; sa.zorig = zorig; sa.tokens = tokens; sa.conf = conf; sa.n0 = n0;
   sa.rowgrp = grp_dev.as<RowGroup>();
   sa.B = B; sa.T = T; sa.C = C; sa.ncc = ncc; sa.V = V; sa.mask_token = mask_token;
+  sa.live = g_dbg_live;
   const SampleDyn* dd = dyn_dev.as<SampleDyn>();
   if (path <= 1) CK(launch_sample_step_dev(sa, dd, st, path == 1));
   else if (path == 2) CK(launch_sample_combine_dev(sa, partials, dd, st));

@@ -49,6 +49,7 @@ struct Args {
   __nv_bfloat16* out;
   const float* rel;
   const int32_t* frames;  // (B) key length of every batch row, null: every row has T
+  const int32_t* live;    // (1) batch rows b >= live[0] are idle this iteration, null: every row is live
   int sat, B, T, H, d;
 };
 
@@ -63,6 +64,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   const int q0 = blockIdx.x * AQ;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
+  if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle row: the whole CTA, before any barrier or TMA work
   // this batch row's own length: keys, queries and stores stop there (rows of a shorter call in a longer launch)
   const int len = a.frames != nullptr ? __ldg(a.frames + b) : a.T;
   if (q0 >= len) return;  // the whole CTA, before any barrier or TMA work
@@ -246,6 +248,7 @@ cudaError_t launch_attention(const AttnPlan& p, cudaStream_t st) {
   a.out = reinterpret_cast<__nv_bfloat16*>(p.out);
   a.rel = p.rel;
   a.frames = p.frames;
+  a.live = p.live;
   a.sat = p.sat; a.B = p.B; a.T = p.T; a.H = p.H; a.d = p.H * att::DH;
   dim3 grid((p.T + att::AQ - 1) / att::AQ, p.H, p.B);
   att::attention_wgmma_kernel<<<grid, att::THREADS, att::SMEM, st>>>(p.tmQ, p.tmK, p.tmVT, a);

@@ -17,8 +17,11 @@ template <bool FROM_CODES>
 __global__ void __launch_bounds__(256) embed_gather_kernel(const int32_t* __restrict__ codes, const float* __restrict__ lat_in,
                                                            const float* __restrict__ table, __nv_bfloat16* __restrict__ A,
                                                            int M, int T, int C, int V1, int K, int Kp,
-                                                           float* __restrict__ ss, int zero_from, int ss_parts) {
-  const long long total = static_cast<long long>(M) * Kp;
+                                                           float* __restrict__ ss, int zero_from, int ss_parts,
+                                                           const int32_t* __restrict__ live) {
+  // rows at or past live[0] * T belong to idle calls (a launch of calls with different step counts): not touched
+  const int m_live = live != nullptr ? min(M, __ldg(live) * T) : M;
+  const long long total = static_cast<long long>(m_live) * Kp;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int m = static_cast<int>(i / Kp), k = static_cast<int>(i - static_cast<long long>(m) * Kp);
@@ -44,7 +47,8 @@ __global__ void __launch_bounds__(256) embed_gather_kernel(const int32_t* __rest
 }
 
 cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, const float* table, void* A, int M, int T,
-                                int C, int V1, int K, int Kp, float* ss, int zero_from, int ss_parts, cudaStream_t st) {
+                                int C, int V1, int K, int Kp, float* ss, int zero_from, int ss_parts,
+                                const int32_t* live, cudaStream_t st) {
   if (K > Kp || ss_parts - zero_from > Kp) return cudaErrorInvalidValue;
   const long long total = static_cast<long long>(M) * Kp;
   long long blocks = (total + 255) / 256;
@@ -53,11 +57,11 @@ cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, 
   if (codes_btc != nullptr)
     embed_gather_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, st>>>(codes_btc, nullptr, table,
                                                                              reinterpret_cast<__nv_bfloat16*>(A), M, T, C, V1, K,
-                                                                             Kp, ss, zero_from, ss_parts);
+                                                                             Kp, ss, zero_from, ss_parts, live);
   else
     embed_gather_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, st>>>(nullptr, latents, nullptr,
                                                                               reinterpret_cast<__nv_bfloat16*>(A), M, T, C, V1,
-                                                                              K, Kp, ss, zero_from, ss_parts);
+                                                                              K, Kp, ss, zero_from, ss_parts, live);
   return cudaGetLastError();
 }
 

@@ -73,7 +73,17 @@ struct GemmArgs {
   // ---- adapted variants (ADAPT): per-row LoRA update of the accumulators, see lora_update() ----
   AdapterRefs lora;
   const int32_t* frames;    // EPI_QKV: (B) frames of every batch row, null = T; v^T columns t >= frames[b] get 0
+  // ---- launches of calls with different step counts: batch rows >= *live (rows >= *live * T) are idle this iteration;
+  // a tile wholly past them does no work, null = every row is live ----
+  const int32_t* live;
 };
+
+// Rows [0, live_rows) of the launch are live: M without a live bound.
+__device__ __forceinline__ int live_rows(const GemmArgs& g) {
+  if (g.live == nullptr) return g.M;
+  const int r = __ldg(g.live) * g.T;
+  return r < g.M ? r : g.M;
+}
 
 __device__ __forceinline__ float gelu_tanh(float x) {
   // 0.5*x*(1+tanh(sqrt(2/pi)*(x+0.044715*x^3)))   (activations.py:16-26); tanh(y) = 1 - 2/(1+exp(2y))
@@ -317,6 +327,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // (the weights, <= 13 MB, stay L2-resident)
   const int m0 = (tile / num_n) * TM + static_cast<int>(rank) * BM;
   const int n0 = (tile % num_n) * BN;
+  // a tile (pair: the cluster's first row, so both CTAs decide alike) past the live rows exits before any barrier or TMA
+  if (g.live != nullptr && (tile / num_n) * TM >= live_rows(g)) return;
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -615,7 +627,8 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
   const int lane = threadIdx.x & 31;
   const int num_n = g.N / BN;
   const int num_kb = g.K / BK;
-  const int tiles = ((g.M + BM - 1) / BM) * num_n;
+  // m-major tile order: the tiles of the live rows are a prefix; every warp role reads the same bound
+  const int tiles = ((live_rows(g) + BM - 1) / BM) * num_n;
   constexpr int kProducer = 8 + GG_EPI_WARPS;
 
   if (warp == kProducer && lane == 0) {
@@ -817,6 +830,7 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
   g.C = p.C; g.ncc = p.ncc; g.V = p.V; g.mask_token = p.mask_token;
   g.lora = p.lora;
   g.frames = p.epi == VNB_EPI_QKV ? p.frames : nullptr;
+  g.live = p.live;
   if (p.lora.table != nullptr) {
     if (!p.lora.grp_adapter || !p.lora.rowgrp || !p.lora.u || p.lora.rows_per_grp < 1) return cudaErrorInvalidValue;
     switch (p.epi) {

@@ -67,8 +67,10 @@ struct AdapterRefs {
   int slot = 0, layer = 0;
   float* u = nullptr;  // (M, R) the down-projection of every adapted row, R = 16 for LORA_QKV ([q | v]), else 8
 };
-// u = y . A'^T for every adapted row of y (M, K) bf16; base rows are not touched
-cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, cudaStream_t st);
+// u = y . A'^T for every adapted row of y (M, K) bf16; base rows are not touched, nor rows at or past live[0] * T
+// (live: device, null = every row)
+cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, const int32_t* live, int T,
+                             cudaStream_t st);
 
 // ---- GEMM ----
 struct GemmPlan {
@@ -96,6 +98,9 @@ struct GemmPlan {
   // VNB_EPI_QKV of a launch whose calls have different lengths: (B) frames of every batch row; v^T column t of batch row
   // b is written as 0 for t >= frames[b] (null: every row has T frames)
   const int32_t* frames = nullptr;
+  // launches of calls with different step counts: (1) the number of live batch rows this iteration (device); tiles
+  // wholly at or past row live[0] * T exit at once (null: every row is live)
+  const int32_t* live = nullptr;
 };
 // Fills the tensor maps; A (M,K) bf16, W (N,K) bf16.
 bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out, void* out2,
@@ -116,6 +121,7 @@ struct AttnPlan {
   void* out = nullptr;         // (B, T, d) bf16
   const float* rel = nullptr;  // (2*sat+1, H)
   const int32_t* frames = nullptr;  // (B) key length of every batch row (device); null: every row has T
+  const int32_t* live = nullptr;    // (1) batch rows b >= live[0] do no work (device); null: every row is live
   int sat = 0, B = 0, T = 0, Tpad = 0, H = 0;
 };
 bool make_attn_plan(AttnPlan* p, const void* qk, const void* vT, void* out, const float* rel, int sat, int B, int T,
@@ -124,9 +130,11 @@ cudaError_t launch_attention(const AttnPlan& p, cudaStream_t st);
 
 // ---- elementwise / gather ----
 // codes_btc (B*T, C) int32 (or latents (B, K, T) fp32 when codes_btc is null) -> A (M, 3*Kp) bf16 = [hi | hi | lo] of the
-// gathered latents, the A operand of the out_proj contraction; zeroes ss partials [zero_from, ss_parts) of every row
+// gathered latents, the A operand of the out_proj contraction; zeroes ss partials [zero_from, ss_parts) of every row.
+// live (device, null = every row): rows at or past live[0] * T are not touched.
 cudaError_t launch_embed_gather(const int32_t* codes_btc, const float* latents, const float* table, void* A, int M, int T,
-                                int C, int V1, int K, int Kp, float* ss, int zero_from, int ss_parts, cudaStream_t st);
+                                int C, int V1, int K, int Kp, float* ss, int zero_from, int ss_parts,
+                                const int32_t* live, cudaStream_t st);
 
 // ---- generate-loop state kernels ----
 // z (B,C,T) int64, mask (B,C,T) int32|null -> zcur (B,T,C) int32 (masked), zorig (B,T,C) int32;
@@ -157,6 +165,7 @@ struct SampleArgs {
   const int32_t* n0;    // (groups) initial mask count of each group
   const RowGroup* rowgrp;  // (B)
   int B, T, C, ncc, V, mask_token;
+  const int32_t* live = nullptr;  // (1) device: batch rows b >= live[0] are idle and left untouched; null = all live
 };
 // use_top_p selects the kernel variant at launch time (it is baked into a captured graph: part of the graph key)
 cudaError_t launch_sample_step_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st, bool use_top_p);

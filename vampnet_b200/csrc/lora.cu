@@ -23,11 +23,15 @@ template <int R> __device__ __forceinline__ int lora_sidx(int k, int j) { return
 
 template <int R>
 __global__ void __launch_bounds__(LORA_THREADS) lora_down_kernel(const __nv_bfloat16* __restrict__ y, int M, int K,
-                                                                  const AdapterRefs r) {
+                                                                  const AdapterRefs r, const int32_t* __restrict__ live,
+                                                                  int T) {
   __shared__ __align__(16) float sA[LORA_KC * R + (LORA_KC / 8) * 4];
+  // rows at or past live[0] * T belong to idle calls (a launch of calls with different step counts): not computed
+  const int m_live = live != nullptr ? min(M, __ldg(live) * T) : M;
+  if (static_cast<int>(blockIdx.x) * LORA_ROWS >= m_live) return;  // the whole block, before any barrier
   const int split = static_cast<int>(threadIdx.x) & (LORA_SPLIT - 1);
   const int m = blockIdx.x * LORA_ROWS + (static_cast<int>(threadIdx.x) >> 2);
-  const int id = m < M ? r.grp_adapter[r.rowgrp[m / r.rows_per_grp].group] : -1;
+  const int id = m < m_live ? r.grp_adapter[r.rowgrp[m / r.rows_per_grp].group] : -1;
   for (int a = 0; a < VNB_MAX_ADAPTERS; ++a) {
     if (!__syncthreads_or(id == a)) continue;
     const float* A = r.table[a].a[r.slot] + static_cast<size_t>(r.layer) * K * R;
@@ -78,13 +82,14 @@ __global__ void __launch_bounds__(LORA_THREADS) lora_down_kernel(const __nv_bflo
   }
 }
 
-cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, cudaStream_t st) {
+cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, const int32_t* live, int T,
+                             cudaStream_t st) {
   if (K % LORA_KC != 0 || M < 1 || !r.table || !r.grp_adapter || !r.rowgrp || !r.u || r.rows_per_grp < 1)
     return cudaErrorInvalidValue;
   const int blocks = (M + LORA_ROWS - 1) / LORA_ROWS;
   const auto* yb = reinterpret_cast<const __nv_bfloat16*>(y);
-  if (r.slot == LORA_QKV) lora_down_kernel<16><<<blocks, LORA_THREADS, 0, st>>>(yb, M, K, r);
-  else lora_down_kernel<8><<<blocks, LORA_THREADS, 0, st>>>(yb, M, K, r);
+  if (r.slot == LORA_QKV) lora_down_kernel<16><<<blocks, LORA_THREADS, 0, st>>>(yb, M, K, r, live, T);
+  else lora_down_kernel<8><<<blocks, LORA_THREADS, 0, st>>>(yb, M, K, r, live, T);
   return cudaGetLastError();
 }
 

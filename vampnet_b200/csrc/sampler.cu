@@ -38,6 +38,7 @@ struct SampleStatic {
   const int32_t* n0;
   const RowGroup* rowgrp;
   int B, T, C, ncc, V, mask_token;
+  const int32_t* live;  // (1) batch rows b >= live[0] are idle this iteration and left untouched; null: all live
 };
 
 // TOPP = false compiles the nucleus filter out (its 32 extra live registers cost occupancy on the common path)
@@ -49,6 +50,7 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
   if (row >= a.B * S) return;
   const int lane = threadIdx.x & 31;
   const int b = row / S, s = row - b * S;
+  if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle call's row: its state is not touched
   const RowGroup rg = a.rowgrp[b];
   const SampleDynDev dyn = dynp[rg.group];
   const uint32_t bg = static_cast<uint32_t>(b - rg.first);  // Philox counter word: the row within its own call
@@ -254,6 +256,7 @@ __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, cons
   const int Cp = a.C - a.ncc;
   const int S = a.T * Cp;
   const int b = blockIdx.x;
+  if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle call's row: zcur is not touched
   const int grp = a.rowgrp[b].group;
   const SampleDynDev dyn = dynp[grp];
   const float* conf = a.conf + static_cast<size_t>(b) * S;
@@ -343,6 +346,7 @@ __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic 
   const int row = blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= a.B * S) return;
   const int b = row / S, s = row - b * S;
+  if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle call's row: tokens and confidences are not touched
   const RowGroup rg = a.rowgrp[b];
   const SampleDynDev dyn = dynp[rg.group];
   const uint32_t bg = static_cast<uint32_t>(b - rg.first);
@@ -409,6 +413,7 @@ static SampleStatic make_static(const SampleArgs& s) {
   a.logits = s.logits; a.zcur = s.zcur; a.zorig = s.zorig; a.tokens = s.tokens; a.conf = s.conf; a.n0 = s.n0;
   a.rowgrp = s.rowgrp;
   a.B = s.B; a.T = s.T; a.C = s.C; a.ncc = s.ncc; a.V = s.V; a.mask_token = s.mask_token;
+  a.live = s.live;
   return a;
 }
 
