@@ -385,6 +385,27 @@ int32_t vnb_codec_conv_in(const float* x, const float* w, const float* bias, con
                           void* stream);
 int32_t vnb_codec_conv_out(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio, int32_t B,
                            int32_t T, int32_t C, int32_t K, int32_t pad, void* stream);
+/* ---- onset detection (reference mask.py:203-226: librosa 0.10 onset.onset_detect(y, sr, hop_length=hop,
+ *      backtrack=True), restated on the device; DESIGN.md §9).  Nothing here synchronises. --------------------------
+ * samples (B, N) fp32 DEVICE, one clip per row; F = 1 + N / hop frames.  Each row is analysed on its own (its own dB
+ * maximum and normalisation), so a row's results equal that row run alone, bit for bit.  Outputs (DEVICE):
+ * envelope (B, F) the normalised onset strength; onsets (B, F) int32, row b's first counts[b] entries are its onset
+ * frames in increasing order (backtrack != 0: moved to the preceding local minimum of the envelope, which may repeat
+ * a frame, as librosa does).  workspace: DEVICE, at least vnb_onset_workspace_bytes(B, N, hop) bytes.  The mel
+ * filterbank, window and FFT twiddles are built on the host in float64 on the first call for a (device, sr, hop) and
+ * cached; that first call allocates and uploads them.  Refused: B outside 1..65535, N < 1, sr < 1, hop < 1, a NULL
+ * buffer, a workspace that is too small. */
+int32_t vnb_onset_workspace_bytes(int32_t B, int32_t N, int32_t hop, uint64_t* bytes);
+int32_t vnb_onset_detect(const float* samples, int32_t B, int32_t N, int32_t sr, int32_t hop, int32_t backtrack,
+                         void* workspace, uint64_t workspace_bytes, float* envelope, int32_t* onsets, int32_t* counts,
+                         void* stream);
+/* mask (B, C, T) int64 DEVICE = the reference's  mask = ones; for idx in onsets: mask[:, :, idx-width:idx+width] = 0
+ * with Python slice semantics (a negative start wraps to T + idx - width, so that slice is usually empty).  Batch
+ * row b uses onset row 0 when onset_rows == 1 (the reference analyses samples[0][0] only), else onset row b; onsets
+ * and counts as written by vnb_onset_detect with F frames per row.  Refused: B, C, T or F < 1, onset_rows not 1 or B,
+ * a NULL buffer. */
+int32_t vnb_onset_mask(const int32_t* onsets, const int32_t* counts, int32_t onset_rows, int32_t F, int32_t width,
+                       int64_t* mask, int32_t B, int32_t C, int32_t T, void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

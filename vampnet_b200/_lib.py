@@ -128,6 +128,11 @@ _SIGS = {
                                         C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,
                                         C.c_void_p, C.c_void_p]),
+    "vnb_onset_workspace_bytes": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    "vnb_onset_detect": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                     C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_onset_mask": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                   C.c_int32, C.c_int32, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
 }

@@ -1103,4 +1103,37 @@ int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, 
   return 0;
 }
 
+// ---- onset detection (onset.cu) ----
+int32_t vnb_onset_workspace_bytes(int32_t B, int32_t N, int32_t hop, uint64_t* bytes) {
+  if (B < 1 || N < 1 || hop < 1 || !bytes) return fail("vnb_onset_workspace_bytes: need B >= 1, N >= 1, hop >= 1 and bytes");
+  *bytes = (uint64_t)B * (uint64_t)(1 + N / hop) * 128u * sizeof(float);
+  return 0;
+}
+int32_t vnb_onset_detect(const float* samples, int32_t B, int32_t N, int32_t sr, int32_t hop, int32_t backtrack,
+                         void* workspace, uint64_t workspace_bytes, float* envelope, int32_t* onsets, int32_t* counts,
+                         void* stream) {
+  if (B < 1 || B > 65535 || N < 1) return fail("vnb_onset_detect: need 1 <= B <= 65535 and N >= 1 (got B = %d, N = %d)", B, N);
+  if (sr < 1 || hop < 1) return fail("vnb_onset_detect: need sr >= 1 and hop >= 1 (got sr = %d, hop = %d)", sr, hop);
+  if (!samples || !workspace || !envelope || !onsets || !counts)
+    return fail("vnb_onset_detect: samples, workspace, envelope, onsets and counts are required");
+  uint64_t need = 0;
+  vnb_onset_workspace_bytes(B, N, hop, &need);
+  if (workspace_bytes < need)
+    return fail("vnb_onset_detect: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
+                (unsigned long long)need);
+  OnsetTables t;
+  CK(onset_tables(sr, hop, &t));
+  CK(launch_onset_detect(samples, B, N, hop, t, reinterpret_cast<float*>(workspace), envelope, onsets, counts,
+                         backtrack != 0, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_onset_mask(const int32_t* onsets, const int32_t* counts, int32_t onset_rows, int32_t F, int32_t width,
+                       int64_t* mask, int32_t B, int32_t C, int32_t T, void* stream) {
+  if (B < 1 || C < 1 || T < 1 || F < 1) return fail("vnb_onset_mask: need B, C, T and F >= 1");
+  if (onset_rows != 1 && onset_rows != B) return fail("vnb_onset_mask: onset_rows must be 1 or B (got %d, B = %d)", onset_rows, B);
+  if (!onsets || !counts || !mask) return fail("vnb_onset_mask: onsets, counts and mask are required");
+  CK(launch_onset_mask(onsets, counts, onset_rows, F, width, mask, B, C, T, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 }  // extern "C"

@@ -174,4 +174,29 @@ cudaError_t launch_sample_combine_dev(const SampleArgs& a, const void* partials,
 // the re-mask alone (the second kernel of both launchers above): reads a.tokens and a.conf, updates a.zcur
 cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st);
 
+// ---- onset detection (onset.cu; librosa 0.10 onset_detect restated, DESIGN.md §9) ----
+// peak_pick windows of onset_detect's defaults at (sr, hop), and the envelope's left padding lag + n_fft // (2 hop)
+struct OnsetGeometry {
+  int pre_max = 0, post_max = 0, pre_avg = 0, post_avg = 0, wait = 0, pad = 0;
+};
+OnsetGeometry onset_geometry(int sr, int hop);
+// device tables (built on the host in float64 once per (device, sr, hop), then cached) and the peak_pick parameters
+struct OnsetTables {
+  const float2* twiddle;   // (1025) exp(-2 pi i k / 2048)
+  const float* window;     // (2048) periodic Hann
+  const float* mel_w;      // nonzero Slaney mel weights, band m at [mel_off[m], mel_off[m + 1])
+  const int32_t* mel_off;  // (129)
+  const int32_t* mel_lo;   // (128) first nonzero bin of band m
+  int pre_max, post_max, pre_avg, post_avg, wait, pad;
+  float delta;
+};
+cudaError_t onset_tables(int sr, int hop, OnsetTables* out);
+// samples (B, N) fp32 -> db_ws (B, F, 128) mel dB, env (B, F) normalised envelope, onsets (B, F) + counts (B)
+cudaError_t launch_onset_detect(const float* samples, int B, int N, int hop, const OnsetTables& t, float* db_ws,
+                                float* env, int32_t* onsets, int32_t* counts, int backtrack, cudaStream_t st);
+// mask (B, C, T) int64: 0 on onset row r's slices [idx - width : idx + width] (Python slice semantics), r = 0 when
+// onset_rows == 1, else r = b; 1 elsewhere
+cudaError_t launch_onset_mask(const int32_t* onsets, const int32_t* counts, int onset_rows, int F, int width,
+                              int64_t* mask, int B, int C, int T, cudaStream_t st);
+
 }  // namespace vnb

@@ -158,7 +158,16 @@ def time_stretch_mask(x: torch.Tensor, stretch_factor: int):
 
 
 def onset_mask(sig, z: torch.Tensor, interface, width: int = 1):
-    """mask.py:203-226 — needs librosa's onset detector, which is outside the hot path (SURVEY.md §2 row 5)."""
+    """mask.py:203-226.  A signal on a CUDA device takes the CUDA detector (vampnet_b200/onset.py: librosa 0.10's
+    onset_detect restated, no host sync); a CPU signal calls librosa's detector as the reference does.  Either way only
+    samples[0][0] is analysed and its onsets apply to every row of z."""
+    if sig.samples.is_cuda:
+        from . import onset
+        det = onset.onset_detect(sig.samples[0][0].detach().float(), sig.sample_rate, interface.codec.hop_length,
+                                 backtrack=True)
+        if z.device != det.frames.device:  # codes held elsewhere: build the mask next to the onsets, then move it
+            return onset.onset_mask(det, z.to(det.frames.device), width).to(z.device)
+        return onset.onset_mask(det, z, width)
     try:
         import librosa
     except ImportError as e:  # pragma: no cover
