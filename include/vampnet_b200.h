@@ -385,6 +385,30 @@ int32_t vnb_codec_conv_in(const float* x, const float* w, const float* bias, con
                           void* stream);
 int32_t vnb_codec_conv_out(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio, int32_t B,
                            int32_t T, int32_t C, int32_t K, int32_t pad, void* stream);
+/* Clips of different lengths in one launch.  The _ragged forms take the arguments above (B, T, Tq: the launch's, i.e.
+ * the longest item's) plus lens, DEVICE int32 [B]: item b's valid OUTPUT rows at this layer's rate (conv_tc: rows of
+ * row_elems elements, N for a plain convolution, Cout for a transposed one, where lens[b] * Cout replaces out_limit;
+ * conv_in / conv_out: samples).  Halo contract, per item b with len = lens[b] and H = 128 rows:
+ *   - rows [0, len) hold the values a launch of that item alone at length len computes, bit for bit, PROVIDED that
+ *     the input rows [len_in, len_in + H) hold +0 (hi and lo) and rows [0, len_in) hold the item's input;
+ *   - conv_tc and conv_in store +0 (fp32, hi and lo) on the rows [len, len + H) (within the output buffer);
+ *   - output rows from len + H on are not written (CTAs whose rows all lie there exit at once), and neither are
+ *     conv_out's samples from len on.
+ * H covers the reach of every codec layer (at most 27 rows), so a chain of ragged layers keeps the contract.  The
+ * edge kernels bound their reads by len, not by zero padding (a tap on +0 could turn a -0 sum into +0).
+ * Refused: a NULL lens, row_elems < 1, and whatever the plain forms refuse. */
+int32_t vnb_codec_conv_tc_ragged(const void* a_hi, const void* a_lo, int32_t B, int32_t Tin, int32_t Cin, int32_t s,
+                                 const void* w_hi, const void* w_lo, int32_t N, int32_t taps, int32_t dil, int32_t pad,
+                                 int32_t Tq, const float* bias, int32_t bias_mod, const float* alpha, int32_t alpha_mod,
+                                 const float* resid, float* out_f32, void* out_hi, void* out_lo,
+                                 int64_t out_batch_stride, int64_t out_offset, int64_t out_limit, int32_t do_tanh,
+                                 const int32_t* lens /* DEVICE [B] */, int32_t row_elems, void* stream);
+int32_t vnb_codec_conv_in_ragged(const float* x, const float* w, const float* bias, const float* alpha, float* out_f32,
+                                 void* out_hi, void* out_lo, int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
+                                 const int32_t* lens /* DEVICE [B] */, void* stream);
+int32_t vnb_codec_conv_out_ragged(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio,
+                                  int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
+                                  const int32_t* lens /* DEVICE [B] */, void* stream);
 /* ---- onset detection (reference mask.py:203-226: librosa 0.10 onset.onset_detect(y, sr, hop_length=hop,
  *      backtrack=True), restated on the device; DESIGN.md §9).  Nothing here synchronises. --------------------------
  * samples (B, N) fp32 DEVICE, one clip per row; F = 1 + N / hop frames.  Each row is analysed on its own (its own dB

@@ -110,6 +110,13 @@ _SIGS = {
                                       C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p]),
     "vnb_codec_conv_in": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_void_p]),
     "vnb_codec_conv_out": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32] * 5 + [C.c_void_p]),
+    "vnb_codec_conv_tc_ragged": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vnb_codec_conv_in_ragged": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]),
+    "vnb_codec_conv_out_ragged": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]),
     "vnb_set_error_cuda": (C.c_int32, [C.c_char_p, C.c_int32]),
     "vnb_dbg_set_live": (C.c_int32, [C.c_void_p]),
     "vnb_dbg_gemm_ref": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),

@@ -25,6 +25,56 @@ import torch.nn as nn
 
 from . import _lib
 
+# Rows x launch samples of one encode_many / decode_many launch: config [3]'s encode, 32 ten-second clips of 441 600
+# samples, so that the peak memory of a mixed launch stays where that batch puts it.
+CODEC_MANY_MAX_SAMPLES = 32 * 441_600
+
+
+def plan_launches(lengths, budget: int = CODEC_MANY_MAX_SAMPLES):
+    """Items (by index) -> launches: longest first (stable), each launch as many items as keep rows x its longest length
+    within `budget` (an item longer than the budget alone still gets a launch of its own)."""
+    order = sorted(range(len(lengths)), key=lambda k: -lengths[k])
+    launches = []
+    for k in order:
+        if launches and (len(launches[-1]) + 1) * lengths[launches[-1][0]] <= budget:
+            launches[-1].append(k)
+        else:
+            launches.append([k])
+    return launches
+
+
+def encoder_lengths(samples, rates):
+    """Valid rows of each item at every rate of the encoder: row 0 audio samples (encoder.conv1 and block 0), row i + 1
+    the output of block i's strided conv; the last row is frames (encoder.conv2 and the quantiser)."""
+    table = [list(samples)]
+    for s in rates:
+        table.append([n // s for n in table[-1]])
+    return table
+
+
+def decoder_lengths(frames, rates):
+    """Valid rows of each item at every rate of the decoder: row 0 frames (decoder.conv1), row i + 1 the output of block
+    i's transposed conv, T * s - s % 2 (ConvTranspose1d(2s, stride s, pad ceil(s/2))); the last row is audio samples."""
+    table = [list(frames)]
+    for s in rates:
+        table.append([t * s - s % 2 for t in table[-1]])
+    return table
+
+
+def upload_lengths(table, device):
+    """(rates, items) int32 on `device`, in one asynchronous copy from pinned memory (no synchronisation)."""
+    host = torch.tensor(table, dtype=torch.int32)
+    if torch.device(device).type != "cuda":
+        return host
+    return host.pin_memory().to(device, non_blocking=True)
+
+
+def zero_frames_past(zc, frames):
+    """zc (B, T, D) channels-last with +0 in every frame t >= frames[b] (frames: int32 [B] on zc's device), one select:
+    the decoder input of a clip coded alone has no such frames, and its first conv reads zeros there."""
+    t = torch.arange(zc.shape[1], device=zc.device, dtype=torch.int32)
+    return torch.where(t.view(1, -1, 1) < frames.view(-1, 1, 1), zc, torch.zeros((), dtype=zc.dtype, device=zc.device))
+
 
 class _Params(nn.Module):
     """Nested parameter holder addressed by dotted names."""
@@ -439,10 +489,107 @@ class DAC(nn.Module):
             audio = self._conv(h, "decoder.conv2", 7, pad=3, alpha=P("decoder.snake1.alpha"), tanh=True)
         return {"audio": audio if length is None else audio[..., :length]}
 
+    # ---- many clips of different lengths -----------------------------------------------------------------------
+    @staticmethod
+    def _refuse_empty(entries, what):
+        if len(entries) == 0:
+            raise ValueError(f"{what}: an empty list")
+        for i, e in enumerate(entries):
+            if e.dim() != 3 or e.shape[0] == 0 or e.shape[-1] == 0:
+                raise ValueError(f"{what}: entry {i} has shape {tuple(e.shape)}; every entry is (B_i >= 1, C, N_i >= 1)")
+
+    @torch.no_grad()
+    def encode_many(self, audio_list, sample_rate=None, budget: int = CODEC_MANY_MAX_SAMPLES):
+        """[encode(a) for a in audio_list], with the rows of all entries sharing launches.  Each entry is (B_i, 1, N_i),
+        N_i a multiple of hop_length (as encode needs, see preprocess); sample_rate: None, one rate, or one per entry
+        (all equal to the codec's).  Rows are sorted longest first and grouped so that rows x launch samples <= budget;
+        a launch runs at its longest row, shorter rows zero-padded, and every row's codes, z and latents equal the
+        row's own encode, bit for bit.  Nothing here synchronises the host."""
+        self._refuse_empty(audio_list, "encode_many")
+        rates = sample_rate if isinstance(sample_rate, (list, tuple)) else [sample_rate] * len(audio_list)
+        if len(rates) != len(audio_list):
+            raise ValueError("encode_many: one sample rate per entry")
+        known = {r for r in rates if r is not None}
+        if len(known) > 1:
+            raise ValueError(f"encode_many: entries of different sample rates {sorted(known)}; resample them first")
+        if known and known != {self.sample_rate}:
+            raise ValueError(f"encode_many: expected {self.sample_rate} Hz, got {known.pop()}")
+        for i, a in enumerate(audio_list):
+            if a.shape[1] != 1 or a.shape[-1] % self.hop_length:
+                raise ValueError(f"encode_many: entry {i} has shape {tuple(a.shape)}; each is (B_i, 1, N_i) with N_i a "
+                                 f"multiple of {self.hop_length} (see preprocess)")
+        if self.precision != "tc":
+            return [self.encode(a) for a in audio_list]
+        items = [(i, j) for i, a in enumerate(audio_list) for j in range(a.shape[0])]
+        samples = [audio_list[i].shape[-1] for i, _ in items]
+        rows = [None] * len(items)
+        for launch in plan_launches(samples, budget):
+            n = samples[launch[0]]
+            x = torch.cat([torch.nn.functional.pad(audio_list[items[k][0]][items[k][1]:items[k][1] + 1]
+                                                   .to(self.device, torch.float32), (0, n - samples[k]))
+                           for k in launch])
+            table = encoder_lengths([samples[k] for k in launch], self.encoder_rates)
+            out = self._encode_launch(x.contiguous(), upload_lengths(table, self.device))
+            for r, k in enumerate(launch):
+                t = table[-1][r]
+                rows[k] = (out["z"][r, :t], out["codes"][r, :, :t], out["latents"][r, :, :t])
+        result, k = [], 0
+        for a in audio_list:
+            mine = rows[k:k + a.shape[0]]
+            k += a.shape[0]
+            zq, codes, lat = (torch.stack([m[f] for m in mine]) for f in range(3))
+            result.append({"z": zq.permute(0, 2, 1), "codes": codes, "latents": lat, "length": a.shape[-1]})
+        return result
+
+    def _encode_launch(self, x, lens):
+        """One ragged encoder launch: x (B, 1, N) -> channels-last z (B, T, D), codes (B, L, T), latents (B, 8L, T)."""
+        self._packed()
+        enc = self._encode_tc(x, lens=lens)
+        return {"z": enc["z"].permute(0, 2, 1), "codes": enc["codes"], "latents": enc["latents"]}
+
+    @torch.no_grad()
+    def decode_many(self, z_list, budget: int = CODEC_MANY_MAX_SAMPLES):
+        """[decode(z) for z in z_list], with the rows of all entries sharing launches.  Each entry is (B_i, D, T_i) with
+        the same D.  Rows are sorted longest first and grouped so that rows x launch samples (frames x hop_length) <=
+        budget; every row's audio equals the row's own decode, bit for bit.  Nothing here synchronises the host."""
+        self._refuse_empty(z_list, "decode_many")
+        dims = {z.shape[1] for z in z_list}
+        if len(dims) > 1:
+            raise ValueError(f"decode_many: entries of different latent counts {sorted(dims)}")
+        if self.precision != "tc":
+            return [self.decode(z) for z in z_list]
+        items = [(i, j) for i, z in enumerate(z_list) for j in range(z.shape[0])]
+        frames = [z_list[i].shape[-1] for i, _ in items]
+        rows = [None] * len(items)
+        D = z_list[0].shape[1]
+        for launch in plan_launches([t * self.hop_length for t in frames], budget):
+            T = frames[launch[0]]
+            # frames past an item's own are left as they are here: the launch's select sets them to +0
+            zc = torch.empty(len(launch), T, D, device=self.device, dtype=torch.float32)
+            for r, k in enumerate(launch):
+                i, j = items[k]
+                zc[r, :frames[k]].copy_(z_list[i][j].transpose(0, 1))
+            table = decoder_lengths([frames[k] for k in launch], self.decoder_rates)
+            audio = self._decode_launch(zc, upload_lengths(table, self.device))
+            for r, k in enumerate(launch):
+                rows[k] = audio[r, :, :table[-1][r]]
+        result, k = [], 0
+        for z in z_list:
+            result.append({"audio": torch.stack(rows[k:k + z.shape[0]])})
+            k += z.shape[0]
+        return result
+
+    def _decode_launch(self, zc, lens):
+        """One ragged decoder launch: zc (B, T, D) channels-last, any values past an item's frames -> audio (B, 1, N)."""
+        self._packed()
+        return self._decode_tc(zc.permute(0, 2, 1), lens=lens)
+
     # ---- tensor-core forward passes (activations channels-last, carried as fp32 stream + hi/lo bf16 operand) ----
     def _tc(self, act, base, N, taps, dil, pad, Tq, s=1, alpha=None, alpha_mod=1, resid=None, out_f32=False,
-            out_split=True, bias_mod=None, out_rows=None, out_offset=0):
-        """One tensor-core convolution.  act = (hi, lo) (B, Tin, Cin).  Returns (f32 | None, (hi, lo) | None)."""
+            out_split=True, bias_mod=None, out_rows=None, out_offset=0, lens=None, zeroed=False):
+        """One tensor-core convolution.  act = (hi, lo) (B, Tin, Cin).  Returns (f32 | None, (hi, lo) | None).
+        lens: DEVICE int32 [B] valid output rows of each item (a ragged launch: vnb_codec_conv_tc_ragged); zeroed: the
+        fp32 output starts as zeros (rows past an item's halo are not written by a ragged launch)."""
         hi, lo = act
         B, Tin, Cin = hi.shape
         wh, wl = self._pack["tc:" + base]
@@ -453,27 +600,36 @@ class DAC(nn.Module):
         # (Tq, s*Cout) view shifted by out_offset
         cout = bias.shape[0]
         shape = (B, out_rows, cout)
-        f32 = resid if resid is not None else (torch.empty(shape, device=dev, dtype=torch.float32) if out_f32 else None)
+        new = torch.zeros if zeroed else torch.empty
+        f32 = resid if resid is not None else (new(shape, device=dev, dtype=torch.float32) if out_f32 else None)
         oh = torch.empty(shape, device=dev, dtype=torch.bfloat16) if out_split else None
         ol = torch.empty(shape, device=dev, dtype=torch.bfloat16) if out_split else None
-        _lib.check(_lib.lib().vnb_codec_conv_tc(
-            _lib.ptr(hi), _lib.ptr(lo), B, Tin, Cin, s, _lib.ptr(wh), _lib.ptr(wl), N, taps, dil, pad, Tq,
-            _lib.ptr(bias), cout if bias_mod is None else bias_mod, _lib.ptr(alpha), alpha_mod, _lib.ptr(resid),
-            _lib.ptr(f32) if (out_f32 or resid is not None) else None, _lib.ptr(oh), _lib.ptr(ol),
-            out_rows * cout, out_offset, out_rows * cout, 0, _lib.stream_ptr(dev)))
+        args = (_lib.ptr(hi), _lib.ptr(lo), B, Tin, Cin, s, _lib.ptr(wh), _lib.ptr(wl), N, taps, dil, pad, Tq,
+                _lib.ptr(bias), cout if bias_mod is None else bias_mod, _lib.ptr(alpha), alpha_mod, _lib.ptr(resid),
+                _lib.ptr(f32) if (out_f32 or resid is not None) else None, _lib.ptr(oh), _lib.ptr(ol),
+                out_rows * cout, out_offset, out_rows * cout, 0)
+        if lens is None:
+            _lib.check(_lib.lib().vnb_codec_conv_tc(*args, _lib.stream_ptr(dev)))
+        else:
+            _lib.check(_lib.lib().vnb_codec_conv_tc_ragged(*args, _lib.ptr(lens), cout, _lib.stream_ptr(dev)))
         return f32, ((oh, ol) if out_split else None)
 
-    def _res_unit_tc(self, skip, act, name, dil, next_alpha):
+    def _res_unit_tc(self, skip, act, name, dil, next_alpha, lens=None):
         """skip: fp32 stream (updated in place); act = split(snake1(skip)); returns split(next_alpha(skip'))."""
         P = self.params.get
         C = skip.shape[-1]
         T = skip.shape[1]
-        _, a2 = self._tc(act, name + ".conv1", C, 7, dil, 3 * dil, T, alpha=P(name + ".snake2.alpha"), alpha_mod=C)
-        _, nxt = self._tc(a2, name + ".conv2", C, 1, 1, 0, T, alpha=next_alpha, alpha_mod=C, resid=skip)
+        _, a2 = self._tc(act, name + ".conv1", C, 7, dil, 3 * dil, T, alpha=P(name + ".snake2.alpha"), alpha_mod=C,
+                         lens=lens)
+        _, nxt = self._tc(a2, name + ".conv2", C, 1, 1, 0, T, alpha=next_alpha, alpha_mod=C, resid=skip, lens=lens)
         return nxt
 
-    def _encode_tc(self, x):
+    def _encode_tc(self, x, lens=None):
+        """x (B, 1, N).  lens: None, or the DEVICE (rates, B) table of encoder_lengths for a launch of items of
+        different lengths (x zero-padded to the longest): each item's rows then equal its own launch, bit for bit,
+        and the outputs past an item's frames are meaningless but finite."""
         P = self.params.get
+        row = (lambda i: None) if lens is None else (lambda i: lens[i])
         B, _, N = x.shape
         lib = _lib.lib()
         with torch.cuda.device(self.device):
@@ -481,10 +637,13 @@ class DAC(nn.Module):
             skip = torch.empty(B, N, d, device=x.device, dtype=torch.float32)
             hi = torch.empty(B, N, d, device=x.device, dtype=torch.bfloat16)
             lo = torch.empty_like(hi)
-            _lib.check(lib.vnb_codec_conv_in(_lib.ptr(x), _lib.ptr(P("encoder.conv1.weight")),
-                                             _lib.ptr(P("encoder.conv1.bias")),
-                                             _lib.ptr(P("encoder.block.0.res_unit1.snake1.alpha")), _lib.ptr(skip),
-                                             _lib.ptr(hi), _lib.ptr(lo), B, N, d, 7, 3, _lib.stream_ptr(x.device)))
+            args = (_lib.ptr(x), _lib.ptr(P("encoder.conv1.weight")), _lib.ptr(P("encoder.conv1.bias")),
+                    _lib.ptr(P("encoder.block.0.res_unit1.snake1.alpha")), _lib.ptr(skip), _lib.ptr(hi), _lib.ptr(lo), B,
+                    N, d, 7, 3)
+            if lens is None:
+                _lib.check(lib.vnb_codec_conv_in(*args, _lib.stream_ptr(x.device)))
+            else:
+                _lib.check(lib.vnb_codec_conv_in_ragged(*args, _lib.ptr(row(0)), _lib.stream_ptr(x.device)))
             act = (hi, lo)
             T = N
             nb = len(self.encoder_rates)
@@ -492,27 +651,35 @@ class DAC(nn.Module):
                 p = f"encoder.block.{i}"
                 for r, dil in enumerate((1, 3, 9)):
                     nxt = P(f"{p}.res_unit{r + 2}.snake1.alpha") if r < 2 else P(p + ".snake1.alpha")
-                    act = self._res_unit_tc(skip, act, f"{p}.res_unit{r + 1}", dil, nxt)
+                    act = self._res_unit_tc(skip, act, f"{p}.res_unit{r + 1}", dil, nxt, lens=row(i))
                 # strided conv: input viewed as (B, T/s, s*C); output feeds the next block (or encoder.snake1)
                 nxt = P(f"encoder.block.{i + 1}.res_unit1.snake1.alpha") if i + 1 < nb else P("encoder.snake1.alpha")
                 skip, act = self._tc(act, p + ".conv1", 2 * d, 2 * s, 1, math.ceil(s / 2), T // s, s=s, alpha=nxt,
-                                     alpha_mod=2 * d, out_f32=(i + 1 < nb))
+                                     alpha_mod=2 * d, out_f32=(i + 1 < nb), lens=row(i + 1))
                 d *= 2
                 T //= s
-            z, _ = self._tc(act, "encoder.conv2", self.latent_dim, 3, 1, 1, T, out_f32=True, out_split=False)
+            # ragged: the quantiser reads every frame of the launch, so frames past an item's halo start as zeros
+            z, _ = self._tc(act, "encoder.conv2", self.latent_dim, 3, 1, 1, T, out_f32=True, out_split=False,
+                            lens=row(nb), zeroed=lens is not None)
             zq_cl, codes, lat = self.quantizer._rvq(0, in_f=z, channels_last=True)
         return {"z": zq_cl.permute(0, 2, 1), "codes": codes, "latents": lat, "length": N}
 
-    def _decode_tc(self, z):
-        """z: (B, latent, T) fp32 (the reference's layout) -> audio (B, 1, T*hop), or shorter for odd decoder rates."""
+    def _decode_tc(self, z, lens=None):
+        """z: (B, latent, T) fp32 (the reference's layout) -> audio (B, 1, T*hop), or shorter for odd decoder rates.
+        lens: None, or the DEVICE (rates, B) table of decoder_lengths for a launch of items of different lengths: frames
+        past an item's own are set to +0 first (one select), and each item's samples then equal its own launch."""
         P = self.params.get
         lib = _lib.lib()
+        row = (lambda i: None) if lens is None else (lambda i: lens[i])
         with torch.cuda.device(self.device):
             zc = z.permute(0, 2, 1).contiguous()  # channels-last
+            if lens is not None:
+                zc = zero_frames_past(zc, lens[0])
             act = self._split(zc)
             B, T, _ = zc.shape
             c = self.decoder_dim
-            _, act = self._tc(act, "decoder.conv1", c, 7, 1, 3, T, alpha=P("decoder.block.0.snake1.alpha"), alpha_mod=c)
+            _, act = self._tc(act, "decoder.conv1", c, 7, 1, 3, T, alpha=P("decoder.block.0.snake1.alpha"), alpha_mod=c,
+                              lens=row(0))
             nb = len(self.decoder_rates)
             for i, s in enumerate(self.decoder_rates):
                 p = f"decoder.block.{i}"
@@ -522,19 +689,23 @@ class DAC(nn.Module):
                 # (T-1)*s - 2*pad + 2*s = T*s - s % 2 rows (ConvTranspose1d), so odd strides drop the last row
                 rows = T * s - s % 2
                 skip, act = self._tc(act, p + ".conv_t1", s * co, 2, -1, 0, T + 1, alpha=P(p + ".res_unit1.snake1.alpha"),
-                                     alpha_mod=co, out_f32=True, bias_mod=co, out_rows=rows, out_offset=-pad * co)
+                                     alpha_mod=co, out_f32=True, bias_mod=co, out_rows=rows, out_offset=-pad * co,
+                                     lens=row(i + 1))
                 T = rows
                 for r, dil in enumerate((1, 3, 9)):
                     if r < 2:
                         nxt = P(f"{p}.res_unit{r + 2}.snake1.alpha")
                     else:
                         nxt = P(f"decoder.block.{i + 1}.snake1.alpha") if i + 1 < nb else P("decoder.snake1.alpha")
-                    act = self._res_unit_tc(skip, act, f"{p}.res_unit{r + 1}", dil, nxt)
+                    act = self._res_unit_tc(skip, act, f"{p}.res_unit{r + 1}", dil, nxt, lens=row(i + 1))
                 c = co
             audio = torch.empty(B, 1, T, device=z.device, dtype=torch.float32)
-            _lib.check(lib.vnb_codec_conv_out(_lib.ptr(act[0]), _lib.ptr(act[1]), _lib.ptr(P("decoder.conv2.weight")),
-                                              _lib.ptr(P("decoder.conv2.bias")), _lib.ptr(audio), B, T, c, 7, 3,
-                                              _lib.stream_ptr(z.device)))
+            args = (_lib.ptr(act[0]), _lib.ptr(act[1]), _lib.ptr(P("decoder.conv2.weight")),
+                    _lib.ptr(P("decoder.conv2.bias")), _lib.ptr(audio), B, T, c, 7, 3)
+            if lens is None:
+                _lib.check(lib.vnb_codec_conv_out(*args, _lib.stream_ptr(z.device)))
+            else:
+                _lib.check(lib.vnb_codec_conv_out_ragged(*args, _lib.ptr(row(nb)), _lib.stream_ptr(z.device)))
         return audio
 
     def forward(self, audio_data, sample_rate=None):

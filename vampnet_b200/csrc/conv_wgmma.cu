@@ -52,7 +52,18 @@ struct ConvTcArgs {
   long long out_offset;         // elements added to q*N + n (negative for transposed convs)
   long long out_limit;          // valid flat range per batch item: [0, out_limit)
   int do_tanh;
+  // Clips of different lengths in one launch (vnb_codec_conv_tc_ragged): DEVICE [Bn] valid output rows of each item,
+  // in rows of row_elems elements (N for a plain convolution, Cout for a transposed one).  NULL: every item is Tq rows.
+  const int* lens; int row_elems;
 };
+
+// Halo of a ragged launch: rows [len_b, len_b + CT_HALO) of every output hold +0, so that the next layer's valid rows
+// read exactly the zeros that TMA's out-of-bounds fill gives a clip coded alone.  The reach past an item's last valid
+// row of each codec layer, in its input rows: k = 7 residual convs 3 * dil <= 27 (dil 1, 3, 9); 1 x 1 convs 0;
+// encoder.conv2 (k 3) 1; decoder.conv1 (k 7) 3; the strided convs (k = 2s, pad ceil(s/2)) one view row, i.e. at most s
+// <= 12 samples; the transposed convs one input row; decoder.conv2 (k 7, codec_out_kernel) 3.
+constexpr int CT_HALO = 128;
+static_assert(CT_HALO >= 27 && CT_HALO >= 12, "the halo covers the largest reach of any codec layer");
 
 // Snake: v + sin^2(a v) / (a + 1e-9).  sin via two-constant Cody-Waite reduction to [-pi, pi] + MUFU.SIN
 // (abs error < 1e-6 for |a v| < 1e4, far below the split-bf16 product error); 1/(a+1e-9) is passed in.
@@ -93,6 +104,16 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
   const int n0 = (tile % n_tiles) * g.BN;
   const int q0 = ((tile / n_tiles) % m_tiles) * CT_BM;
   const int b = tile / n_tiles / m_tiles;
+  // stores are kept to flat indices [0, store_limit); values to [0, value_limit), the rest of that range gets +0
+  long long value_limit = g.out_limit, store_limit = g.out_limit;
+  if (g.lens != nullptr) {
+    const long long len = g.lens[b];
+    const long long halo_end = (len + CT_HALO) * g.row_elems;
+    // no output row of this tile lies below the halo's end (block-uniform): nothing to load, compute or store
+    if (static_cast<long long>(q0) * g.N + g.out_offset >= halo_end) return;
+    value_limit = min(len * g.row_elems, g.out_limit);
+    store_limit = min(halo_end, g.out_limit);
+  }
 
   if (warp == CT_EPI_WARPS && lane == 0) {
     tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
@@ -235,7 +256,9 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
 #pragma unroll
       for (int itr = 0; itr < 8; ++itr) {
         const long long flat = flat0 + itr * row_step;
-        if (q + 4 * itr < g.Tq && flat >= 0 && flat < g.out_limit) {
+        if (q + 4 * itr < g.Tq && flat >= 0 && flat < store_limit) {
+          // halo rows of a ragged launch: +0 by a select (padded rows may have accumulated NaN), never a product
+          const bool halo = flat >= value_limit;
           const uint32_t sp = sp0 + 4u * (itr * 4 * CT_ACC_PITCH);
           float4 a = make_float4(lds_f32(sp) + bv.x, lds_f32(sp + 4) + bv.y, lds_f32(sp + 8) + bv.z,
                                  lds_f32(sp + 12) + bv.w);
@@ -245,6 +268,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
             a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
           }
           if (do_tanh) { a.x = tanhf(a.x); a.y = tanhf(a.y); a.z = tanhf(a.z); a.w = tanhf(a.w); }
+          if (halo) a = make_float4(0.f, 0.f, 0.f, 0.f);
           if (out_f32) *reinterpret_cast<float4*>(g.out_f32 + o) = a;
           if (out_split) {
             if (snake) {
@@ -258,6 +282,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
             hi.y = *reinterpret_cast<const uint32_t*>(&h23);
             lo.x = pack_bf16x2(a.x - f01.x, a.y - f01.y);
             lo.y = pack_bf16x2(a.z - f23.x, a.w - f23.y);
+            if (halo) { hi = make_uint2(0u, 0u); lo = make_uint2(0u, 0u); }
             *reinterpret_cast<uint2*>(g.out_hi + o) = hi;
             *reinterpret_cast<uint2*>(g.out_lo + o) = lo;
           }
@@ -281,18 +306,27 @@ __global__ void __launch_bounds__(256) codec_in_kernel(const float* __restrict__
                                                        const float* __restrict__ bias, const float* __restrict__ alpha,
                                                        float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_hi,
                                                        __nv_bfloat16* __restrict__ out_lo, int B, int T, int C, int K,
-                                                       int pad) {
+                                                       int pad, const int* __restrict__ lens) {
   const int C4 = C >> 2;                                  // threads per frame
   const int per_block = blockDim.x / C4;                  // frames per block (host guarantees divisibility)
   const int t = blockIdx.x * per_block + static_cast<int>(threadIdx.x) / C4, b = blockIdx.y;
   if (t >= T) return;
+  const int Tb = lens != nullptr ? lens[b] : T;           // this item's samples (ragged launch) or the launch's
+  if (t >= Tb + CT_HALO) return;
   const int c = (static_cast<int>(threadIdx.x) % C4) * 4;
   const long long bt = static_cast<long long>(b) * T + t;
+  if (t >= Tb) {                                          // halo of a ragged launch: +0 in all three outputs
+    const long long o = bt * C + c;
+    *reinterpret_cast<float4*>(out_f32 + o) = make_float4(0.f, 0.f, 0.f, 0.f);
+    *reinterpret_cast<uint2*>(out_hi + o) = make_uint2(0u, 0u);
+    *reinterpret_cast<uint2*>(out_lo + o) = make_uint2(0u, 0u);
+    return;
+  }
   const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + c));
   float acc[4] = {b4.x, b4.y, b4.z, b4.w};
   for (int k = 0; k < K; ++k) {
     const int xi = t + k - pad;
-    if (xi >= 0 && xi < T) {
+    if (xi >= 0 && xi < Tb) {
       const float xv = __ldg(x + static_cast<long long>(b) * T + xi);
 #pragma unroll
       for (int j = 0; j < 4; ++j) acc[j] = fmaf(__ldg(w + (c + j) * K + k), xv, acc[j]);
@@ -324,11 +358,12 @@ constexpr int CO_K = 7;
 __global__ void __launch_bounds__(256) codec_out_kernel(const __nv_bfloat16* __restrict__ ah,
                                                         const __nv_bfloat16* __restrict__ al, const float* __restrict__ w,
                                                         const float* __restrict__ bias, float* __restrict__ audio, int B,
-                                                        int T, int C, int pad) {
+                                                        int T, int C, int pad, const int* __restrict__ lens) {
   const int lane = threadIdx.x & 31;
   const int t0 = (blockIdx.x * 8 + (threadIdx.x >> 5)) * 32;
   const int b = blockIdx.y;
-  if (t0 >= T) return;
+  const int Tb = lens != nullptr ? lens[b] : T;   // this item's samples (ragged launch: input frames past it are not read)
+  if (t0 >= Tb) return;
   const int c = lane * 4;
   const bool lane_on = c < C;
   float wr[4][CO_K];  // weight (1, C, K) -> this lane's [channel][tap]
@@ -347,7 +382,7 @@ __global__ void __launch_bounds__(256) codec_out_kernel(const __nv_bfloat16* __r
     const int t = t0 - pad + r;   // input frame; it is tap k of output r - k
     // unconditional loads from a clamped address (no branch between the loads: they are issued back to back and
     // their latency overlaps); frames outside the clip and idle lanes contribute zeros
-    const bool ok = lane_on && t >= 0 && t < T;
+    const bool ok = lane_on && t >= 0 && t < Tb;
     const long long off = static_cast<long long>(ok ? t : 0) * C;
     const uint2 h = __ldg(reinterpret_cast<const uint2*>(ph + off));
     const uint2 l = __ldg(reinterpret_cast<const uint2*>(pl + off));
@@ -380,7 +415,7 @@ __global__ void __launch_bounds__(256) codec_out_kernel(const __nv_bfloat16* __r
     }
   }
   const int t = t0 + lane;
-  if (t < T) audio[static_cast<long long>(b) * T + t] = tanhf(bias[0] + acc[0]);
+  if (t < Tb) audio[static_cast<long long>(b) * T + t] = tanhf(bias[0] + acc[0]);
 }
 
 // Opts the four epilogue variants of width NW in to the large shared memory (once per device) and launches the one
@@ -415,13 +450,12 @@ static cudaError_t launch_conv(const CUtensorMap& tAh, const CUtensorMap& tAl, c
 }  // namespace vnb
 
 using namespace vnb;
-extern "C" {
 
-int32_t vnb_codec_conv_tc(const void* a_hi, const void* a_lo, int32_t B, int32_t Tin, int32_t Cin, int32_t s,
-                          const void* w_hi, const void* w_lo, int32_t N, int32_t taps, int32_t dil, int32_t pad,
-                          int32_t Tq, const float* bias, int32_t bias_mod, const float* alpha, int32_t alpha_mod,
-                          const float* resid, float* out_f32, void* out_hi, void* out_lo, int64_t out_batch_stride,
-                          int64_t out_offset, int64_t out_limit, int32_t do_tanh, void* stream) {
+static int32_t conv_tc(const void* a_hi, const void* a_lo, int32_t B, int32_t Tin, int32_t Cin, int32_t s,
+                       const void* w_hi, const void* w_lo, int32_t N, int32_t taps, int32_t dil, int32_t pad, int32_t Tq,
+                       const float* bias, int32_t bias_mod, const float* alpha, int32_t alpha_mod, const float* resid,
+                       float* out_f32, void* out_hi, void* out_lo, int64_t out_batch_stride, int64_t out_offset,
+                       int64_t out_limit, int32_t do_tanh, const int32_t* lens, int32_t row_elems, void* stream) {
   if (Tin % s != 0) return vnb_set_error_cuda("vnb_codec_conv_tc: Tin must be a multiple of the stride", 1);
   if (N % 32 != 0 || Cin % 4 != 0) return vnb_set_error_cuda("vnb_codec_conv_tc: N % 32 and Cin % 4 required", 1);
   ConvTcArgs g;
@@ -432,6 +466,7 @@ int32_t vnb_codec_conv_tc(const void* a_hi, const void* a_lo, int32_t B, int32_t
   g.bias = bias; g.bias_mod = bias_mod; g.alpha = alpha; g.alpha_mod = alpha_mod; g.resid = resid; g.out_f32 = out_f32;
   g.out_hi = reinterpret_cast<__nv_bfloat16*>(out_hi); g.out_lo = reinterpret_cast<__nv_bfloat16*>(out_lo);
   g.out_batch_stride = out_batch_stride; g.out_offset = out_offset; g.out_limit = out_limit; g.do_tanh = do_tanh;
+  g.lens = lens; g.row_elems = row_elems;
   const int Ktot = taps * g.cblocks * CT_BK;
   CUtensorMap tAh, tAl, tWh, tWl;
   const uint64_t rows = static_cast<uint64_t>(Tin / s), cols = static_cast<uint64_t>(s) * Cin;
@@ -446,30 +481,78 @@ int32_t vnb_codec_conv_tc(const void* a_hi, const void* a_lo, int32_t B, int32_t
   return 0;
 }
 
-int32_t vnb_codec_conv_in(const float* x, const float* w, const float* bias, const float* alpha, float* out_f32,
-                          void* out_hi, void* out_lo, int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
-                          void* stream) {
+static int32_t conv_in(const float* x, const float* w, const float* bias, const float* alpha, float* out_f32,
+                       void* out_hi, void* out_lo, int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
+                       const int32_t* lens, void* stream) {
   if (C % 4 != 0 || 256 % (C / 4) != 0) return vnb_set_error_cuda("vnb_codec_conv_in: C/4 must divide 256", 1);
   const int per_block = 256 / (C / 4);
   dim3 grid((T + per_block - 1) / per_block, B);
   codec_in_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, w, bias, alpha, out_f32, reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), B, T,
-      C, K, pad);
+      C, K, pad, lens);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) count_launch();
   return e == cudaSuccess ? 0 : vnb_set_error_cuda("codec_in_kernel", static_cast<int>(e));
 }
 
-int32_t vnb_codec_conv_out(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio, int32_t B,
-                           int32_t T, int32_t C, int32_t K, int32_t pad, void* stream) {
+static int32_t conv_out(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio, int32_t B,
+                        int32_t T, int32_t C, int32_t K, int32_t pad, const int32_t* lens, void* stream) {
   if (K != CO_K || C % 4 != 0 || C > 128)
     return vnb_set_error_cuda("vnb_codec_conv_out: kernel size 7 and C % 4 == 0, C <= 128 required", 1);
   dim3 grid((T + 255) / 256, B);
   codec_out_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(a_hi), reinterpret_cast<const __nv_bfloat16*>(a_lo), w, bias, audio, B, T, C,
-      pad);
+      pad, lens);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) count_launch();
   return e == cudaSuccess ? 0 : vnb_set_error_cuda("codec_out_kernel", static_cast<int>(e));
+}
+
+extern "C" {
+
+int32_t vnb_codec_conv_tc(const void* a_hi, const void* a_lo, int32_t B, int32_t Tin, int32_t Cin, int32_t s,
+                          const void* w_hi, const void* w_lo, int32_t N, int32_t taps, int32_t dil, int32_t pad,
+                          int32_t Tq, const float* bias, int32_t bias_mod, const float* alpha, int32_t alpha_mod,
+                          const float* resid, float* out_f32, void* out_hi, void* out_lo, int64_t out_batch_stride,
+                          int64_t out_offset, int64_t out_limit, int32_t do_tanh, void* stream) {
+  return conv_tc(a_hi, a_lo, B, Tin, Cin, s, w_hi, w_lo, N, taps, dil, pad, Tq, bias, bias_mod, alpha, alpha_mod, resid,
+                 out_f32, out_hi, out_lo, out_batch_stride, out_offset, out_limit, do_tanh, nullptr, 0, stream);
+}
+
+int32_t vnb_codec_conv_tc_ragged(const void* a_hi, const void* a_lo, int32_t B, int32_t Tin, int32_t Cin, int32_t s,
+                                 const void* w_hi, const void* w_lo, int32_t N, int32_t taps, int32_t dil, int32_t pad,
+                                 int32_t Tq, const float* bias, int32_t bias_mod, const float* alpha, int32_t alpha_mod,
+                                 const float* resid, float* out_f32, void* out_hi, void* out_lo,
+                                 int64_t out_batch_stride, int64_t out_offset, int64_t out_limit, int32_t do_tanh,
+                                 const int32_t* lens, int32_t row_elems, void* stream) {
+  if (lens == nullptr || row_elems < 1)
+    return vnb_set_error_cuda("vnb_codec_conv_tc_ragged: a length table and row_elems >= 1 required", 1);
+  return conv_tc(a_hi, a_lo, B, Tin, Cin, s, w_hi, w_lo, N, taps, dil, pad, Tq, bias, bias_mod, alpha, alpha_mod, resid,
+                 out_f32, out_hi, out_lo, out_batch_stride, out_offset, out_limit, do_tanh, lens, row_elems, stream);
+}
+
+int32_t vnb_codec_conv_in(const float* x, const float* w, const float* bias, const float* alpha, float* out_f32,
+                          void* out_hi, void* out_lo, int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
+                          void* stream) {
+  return conv_in(x, w, bias, alpha, out_f32, out_hi, out_lo, B, T, C, K, pad, nullptr, stream);
+}
+
+int32_t vnb_codec_conv_in_ragged(const float* x, const float* w, const float* bias, const float* alpha, float* out_f32,
+                                 void* out_hi, void* out_lo, int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad,
+                                 const int32_t* lens, void* stream) {
+  if (lens == nullptr) return vnb_set_error_cuda("vnb_codec_conv_in_ragged: a length table is required", 1);
+  return conv_in(x, w, bias, alpha, out_f32, out_hi, out_lo, B, T, C, K, pad, lens, stream);
+}
+
+int32_t vnb_codec_conv_out(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio, int32_t B,
+                           int32_t T, int32_t C, int32_t K, int32_t pad, void* stream) {
+  return conv_out(a_hi, a_lo, w, bias, audio, B, T, C, K, pad, nullptr, stream);
+}
+
+int32_t vnb_codec_conv_out_ragged(const void* a_hi, const void* a_lo, const float* w, const float* bias, float* audio,
+                                  int32_t B, int32_t T, int32_t C, int32_t K, int32_t pad, const int32_t* lens,
+                                  void* stream) {
+  if (lens == nullptr) return vnb_set_error_cuda("vnb_codec_conv_out_ragged: a length table is required", 1);
+  return conv_out(a_hi, a_lo, w, bias, audio, B, T, C, K, pad, lens, stream);
 }
 }

@@ -198,6 +198,22 @@ class Interface(torch.nn.Module):
         signal = self._preprocess(signal)
         return self.codec.encode(signal.samples, signal.sample_rate)["codes"]
 
+    def decode_many(self, z_list: list):
+        """[decode(z) for z in z_list], bit for bit, with the codec's decoder run over all entries together (clips of
+        different lengths share launches)."""
+        return self.coarse.decode_many(z_list, self.codec)
+
+    @torch.inference_mode()
+    def encode_many(self, signals: list):
+        """[encode(s) for s in signals], bit for bit: each signal is preprocessed as encode does (resample, mono,
+        loudness, peak, hop padding), then the codec's encoder runs over all of them together (clips of different
+        lengths share launches)."""
+        if len(signals) == 0:
+            raise ValueError("encode_many: an empty list")
+        prepared = [self._preprocess(s.to(self.device)) for s in signals]
+        enc = self.codec.encode_many([s.samples for s in prepared], [s.sample_rate for s in prepared])
+        return [e["codes"] for e in enc]
+
     def make_beat_mask(self, *a, **k):
         raise RuntimeError("make_beat_mask needs the WaveBeat tracker (interface.py:226-322), a separate model "
                            "outside the hot path (SURVEY.md §2 row 9)")

@@ -868,3 +868,20 @@ class VampNet(nn.Module):
         from ..audio import AudioSignal
         zq = codec.quantizer.from_latents(self.embedding.from_codes(z, codec))[0]
         return AudioSignal(codec.decode(zq)["audio"], codec.sample_rate)
+
+    @torch.no_grad()
+    def decode_many(self, z_list, codec):
+        """[decode(z, codec) for z in z_list], bit for bit, with the codec's decoder run over the rows of all entries
+        together (DAC.decode_many: clips of different lengths share launches).  Entries are (B_i, n_codebooks, T_i) codes
+        with the same codebook count."""
+        if len(z_list) == 0:
+            raise ValueError("decode_many: an empty list")
+        books = {z.shape[1] if z.ndim == 3 else None for z in z_list}
+        if None in books:
+            raise ValueError("decode_many: every entry is (B_i, n_codebooks, T_i)")
+        if len(books) > 1:
+            raise ValueError(f"decode_many: entries of different codebook counts {sorted(books)}")
+        from ..audio import AudioSignal
+        zq = [codec.quantizer.from_latents(self.embedding.from_codes(z.masked_fill(z == self.mask_token, 0), codec))[0]
+              for z in z_list]
+        return [AudioSignal(d["audio"], codec.sample_rate) for d in codec.decode_many(zq)]
