@@ -203,6 +203,22 @@ int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, 
                            const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
                            int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
                            int32_t use_graph, int64_t* out, void* stream);
+/* vnb_generate_steps for groups that may mix nucleus (top-p) and plain sampling: same arguments, same contract, and each
+ * group's out equals, bit for bit, vnb_generate_steps of its rows alone.  A group's top-p is on when 0 < top_p < 1.
+ *   every group on, or every group off: vnb_generate_steps's kernels and graph;
+ *   a mix, "fused_sampler" 1 (and a vocabulary the fused sampler takes): the classifier's split sampling epilogue writes
+ *     the records of the plain groups' still-masked positions and stores the fp32 logits of the nucleus groups'
+ *     still-masked positions; then the plain rows draw from the records (sample_combine_kernel) and the nucleus rows
+ *     from the logits (sample_rows_kernel with the filter), each kernel touching its own rows only; then the re-mask;
+ *   a mix, "fused_sampler" 0: the materialising path with the nucleus kernel for every row (a group whose top-p is off
+ *     draws there exactly as it does without the filter).
+ * The group -> top-p assignment is read from the per-step table written before every launch or replay: one
+ * (B, T, S) graph serves any mix.  The logits tensor (M x (C - ncc) x V fp32) is allocated whenever a group's top-p is
+ * on.  Errors: those of vnb_generate_steps except the mix. */
+int32_t vnb_generate_mixed_top_p(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                 const int32_t* group_steps, const float* const* group_gamma,
+                                 const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
+                                 const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream);
 /* One sampling iteration on caller-supplied logits (B, S, V) fp32 — sample_from_logits +
  * mask_by_random_topk + the where()s around them (transformer.py:849-932).  State is explicit:
  * zflat (B, S) int32 in "t c" order (util.py:39) is updated in place; tokens_out (B, S) int32
@@ -218,9 +234,9 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
  * number of kernel nodes it contains).
  * vnb_graph_capture_count: generate graphs captured so far (a weight hot swap or a repeated call must not
  * add to it: graphs are cached per (workspace, steps, mask, top_p, adapted or not, some group shorter than T or
- * not, some group with fewer steps than the launch or not); the grouping of vnb_generate_many, the group -> adapter
- * table, the per-row frames of vnb_generate_ragged and the step counts of vnb_generate_steps are not part of that
- * key).
+ * not, some group with fewer steps than the launch or not, nucleus and plain groups in one fused launch or not); the
+ * grouping of vnb_generate_many, the group -> adapter table, the per-row frames of vnb_generate_ragged, the step counts
+ * of vnb_generate_steps and the group -> top-p assignment of vnb_generate_mixed_top_p are not part of that key).
  * vnb_profile_begin/end: between the two calls every launch of forward/generate is bracketed by CUDA
  * events on the launching stream (graph replay is bypassed so that the events can be recorded);
  * end() returns the summed device time and launch count per kernel family:
@@ -239,7 +255,8 @@ uint64_t vnb_graph_capture_count(void);
  *              compiled default.  Generate graphs are cached per value.
  * "fused_sampler": 1 (default) = vnb_generate samples inside the classifier GEMM's epilogue (VNB_EPI_SAMPLE: the logits of
  *   the generate loop never reach HBM), 0 = from a materialised fp32 logits tensor (sample_rows_kernel).  Both draw
- *   with the same two-level inverse CDF and the same Philox stream; nucleus (top-p) sampling always materialises.
+ *   with the same two-level inverse CDF and the same Philox stream; nucleus (top-p) sampling always draws from
+ *   materialised logits (in a fused vnb_generate_mixed_top_p launch, those the split epilogue stores for its rows).
  * "gemm_pair_max_clusters" (get only): clusters of two that can be co-resident on the current device. */
 int32_t vnb_set_option(const char* name, int32_t value);
 int32_t vnb_get_option(const char* name, int32_t* value);
@@ -347,6 +364,25 @@ typedef struct vnb_sample_group {
 int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
                        int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
                        int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream);
+/* Test-only: the classifier GEMM with the split sampling epilogue of a fused vnb_generate_mixed_top_p launch.  The
+ * arguments of vnb_dbg_gemm_sample, except that the per-call scalars come from groups[n_groups] over the M / T batch rows
+ * (M a multiple of T; temperature, do_sample, step, seeds and top_p are read), plus logits (M, N) fp32.  A still-masked
+ * position of a plain group (top_p <= 0 or >= 1) gets the record vnb_dbg_gemm_sample writes; one of a nucleus group gets
+ * no record, and its 128-column strip of logits is stored at logits[m*N + (cp*V + v)] with the bits of
+ * vnb_dbg_gemm_fused(VNB_EPI_BIAS_F32).  Nothing else is written.  Synchronises `stream` before returning. */
+int32_t vnb_dbg_gemm_sample_split(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,
+                                  const float* ss_in, int32_t ss_parts, float inv_d, float eps, const int32_t* zcur,
+                                  int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token,
+                                  const vnb_sample_group* groups, int32_t n_groups, void* partials, float* logits,
+                                  void* stream);
+/* Test-only: the sampler of a fused vnb_generate_mixed_top_p launch, with vnb_dbg_sample's arguments and rules: the
+ * combine (path 2) on the rows of plain groups from partials, the nucleus draw (path 1) on the rows of nucleus groups
+ * from logits, each leaving the other kind's tokens and conf untouched, then the re-mask of every row.  Both partials
+ * and logits are required. */
+int32_t vnb_dbg_sample_split(const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                             int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C,
+                             int32_t ncc, int32_t V, int32_t mask_token, const vnb_sample_group* groups,
+                             int32_t n_groups, void* stream);
 
 /* ---- codec (DAC family; reference call sites: interface.py:223 codec.encode, transformer.py:671-675
  *      codec.quantizer.from_latents + codec.decode).  fp32, (B, C, T) channels-first. ------------------------

@@ -83,6 +83,10 @@ _SIGS = {
     "vnb_generate_steps": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
                                        C.POINTER(C.POINTER(C.c_float)), C.POINTER(GenGroup), C.c_int32,
                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_generate_mixed_top_p": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_int32), C.POINTER(C.POINTER(C.c_float)), C.POINTER(GenGroup),
+                                             C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                             C.c_void_p, C.c_void_p]),
     "vnb_adapter_add": (C.c_int32, [C.c_void_p, C.POINTER(AdapterWeights), C.POINTER(C.c_int32)]),
     "vnb_adapter_remove": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vnb_forward_codes_adapted": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
@@ -142,6 +146,12 @@ _SIGS = {
                                    C.c_int32, C.c_int32, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
+    "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,
+                                                                             C.c_void_p]),
+    "vnb_dbg_gemm_sample_split": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_int32,
+                                              C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(SampleGroup),
+                                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -142,9 +142,10 @@ struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in w
   bool adapted;  // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
   bool ragged;   // QKV and attention read the frames table (some group is shorter than T)
   bool mixed_steps;  // every kernel of iteration i reads the live table (some group has fewer steps than the launch)
+  bool split;        // nucleus and plain groups in one fused launch: split classifier epilogue and sampler
   bool operator<(const GraphKey& o) const {
-    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged, mixed_steps) <
-           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged, o.mixed_steps);
+    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged, mixed_steps, split) <
+           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged, o.mixed_steps, o.split);
   }
 };
 
@@ -363,9 +364,11 @@ static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int 
   return 0;
 }
 
-// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  ragged: batch row b
-// is a call of ws->frames[b] frames; its later frames are padding that no earlier frame attends to.  live (device, null
-// = every row): batch rows at or past live[0] are idle; every kernel skips the tiles and CTAs wholly past them.
+// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  fused_dyn: the
+// classifier samples in its epilogue instead; with `logits` as well, the split epilogue stores the logits of the rows of
+// nucleus (top-p) groups there.  ragged: batch row b is a call of ws->frames[b] frames; its later frames are padding
+// that no earlier frame attends to.  live (device, null = every row): batch rows at or past live[0] are idle; every
+// kernel skips the tiles and CTAs wholly past them.
 static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st, float* acts = nullptr,
                      const SampleDyn* fused_dyn = nullptr, bool adapted = false, bool ragged = false,
                      const int32_t* live = nullptr) {
@@ -397,6 +400,10 @@ static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st
   if (fused_dyn != nullptr) {  // generate loop: sample in the classifier's epilogue, no logits tensor
     GemmPlan cls = bounded(ws->cls_sample);
     cls.dyn = fused_dyn;
+    if (logits != nullptr) {
+      cls.out = logits;
+      cls.sample_split = true;
+    }
     LAUNCH(FAM_GEMM_CLS, launch_gemm(cls, st));
   } else {
     GemmPlan cls = bounded(ws->cls);
@@ -589,7 +596,8 @@ int32_t vnb_get_hidden(vnb_model* m, float* out, void* stream) {
 }
 
 // vnb_set_option("fused_sampler", 0|1): sample inside the classifier GEMM's epilogue (default) or from a materialised
-// logits tensor.  Nucleus (top-p) filtering needs whole sorted rows and always takes the materialising path.
+// logits tensor.  Nucleus (top-p) filtering needs whole sorted rows: its rows always draw from materialised logits (in a
+// fused launch of nucleus and plain groups, from those the split classifier epilogue stores).
 static int g_fused_sampler = -1;  // -1: not read yet (environment VNB_FUSED_SAMPLER, else on)
 static int fused_sampler_enabled() {
   if (g_fused_sampler < 0) {
@@ -600,8 +608,11 @@ static int fused_sampler_enabled() {
 }
 
 // mixed_steps: iteration i runs only the batch rows ws->live[i] counts (a prefix); the others are idle and untouched.
+// split (with fused): nucleus and plain groups; the classifier stores the nucleus rows' logits, and the sampler runs the
+// combine for the plain rows and the nucleus draw for the others.
 static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int steps, int64_t* out,
-                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged, bool mixed_steps) {
+                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged, bool mixed_steps,
+                            bool split) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
   // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
@@ -621,7 +632,11 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
     sa.live = live;
     if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st, live)) return 1;
     const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
-    if (fused) {
+    if (split) {
+      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, dyn_i, adapted, ragged, live)) return 1;
+      LAUNCH(FAM_SAMPLE, launch_sample_split_dev(sa, ws->partials.p, dyn_i, st));
+      ++g_launches;  // the split sampler is one kernel more
+    } else if (fused) {
       if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted, ragged, live)) return 1;
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
     } else {
@@ -637,27 +652,35 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
 
 }  // extern "C"
 
-// The launch behind vnb_generate_ragged and vnb_generate_steps: group g runs group_steps[g] steps (NULL: every group
-// runs `steps`) with its own gamma schedule group_gamma[g] (NULL: every group uses `gamma`).  The caller has checked the
-// steps and their order; `steps` is their maximum S.  Group g is idle for the first S - steps_g iterations and then runs
-// its own step j = i - (S - steps_g) with j's schedule values, Philox step word and last-step flag.
+// The launch behind vnb_generate_ragged, vnb_generate_steps and vnb_generate_mixed_top_p: group g runs group_steps[g]
+// steps (NULL: every group runs `steps`) with its own gamma schedule group_gamma[g] (NULL: every group uses `gamma`).
+// The caller has checked the steps and their order; `steps` is their maximum S.  Group g is idle for the first
+// S - steps_g iterations and then runs its own step j = i - (S - steps_g) with j's schedule values, Philox step word and
+// last-step flag.  mixed_top_p: groups may mix nucleus (top-p) and plain sampling, each row drawing as its group's own
+// launch would.
 static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
                            const float* gamma, const int32_t* group_steps, const float* const* group_gamma,
                            const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
-                           const int32_t* group_adapter, int32_t use_graph, int64_t* out, cudaStream_t st) {
+                           const int32_t* group_adapter, int32_t use_graph, int64_t* out, cudaStream_t st,
+                           bool mixed_top_p = false) {
   if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
   if ((!gamma && !group_gamma) || !groups) return fail("vnb_generate_many: gamma and groups are required");
   if (B < 1 || T < 1) return fail("vnb_generate_many: need B >= 1 and T >= 1 (got %d, %d)", B, T);
   if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
   const auto top_p_on = [](float tp) { return tp > 0.f && tp < 1.f; };
-  const bool use_top_p = top_p_on(groups[0].top_p);
+  bool use_top_p = top_p_on(groups[0].top_p), top_p_mix = false;
   long long total = 0;
   for (int g = 0; g < n_groups; ++g) {
     const vnb_gen_group& q = groups[g];
     if (q.rows < 1) return fail("vnb_generate_many: group %d has %d rows", g, q.rows);
     if (!q.temp_eff || !q.do_sample) return fail("vnb_generate_many: group %d lacks its schedules", g);
-    // the sampler variant is chosen per launch: a mixed launch would filter differently from the separate calls
-    if (top_p_on(q.top_p) != use_top_p) return fail("vnb_generate_many: groups mix top-p and no top-p sampling");
+    // outside vnb_generate_mixed_top_p the sampler variant is chosen per launch: a mixed launch would filter
+    // differently from the separate calls
+    if (top_p_on(q.top_p) != top_p_on(groups[0].top_p)) {
+      if (!mixed_top_p) return fail("vnb_generate_many: groups mix top-p and no top-p sampling");
+      top_p_mix = true;
+      use_top_p = true;
+    }
     total += q.rows;
   }
   if (total != B) return fail("vnb_generate_many: group rows sum to %lld, not B = %d", total, B);
@@ -713,11 +736,14 @@ static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, 
   if (ragged) CK(cudaMemcpyAsync(ws->frames.p, frames.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
   if (mixed_steps) CK(cudaMemcpyAsync(ws->live.p, live.data(), sizeof(int32_t) * steps, cudaMemcpyHostToDevice, st));
   if (adapted && stage_adapters(m, ws, group_adapter, n_groups, st)) return 1;
-  const bool fused = fused_sampler_enabled() != 0 && !use_top_p && ws->can_fuse;
-  if (!fused && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
+  // a mix of nucleus and plain groups: the split path when the sampler is fused, else the materialising path with the
+  // nucleus kernel for every row (a group whose top-p is off draws there as without the filter, bit for bit)
+  const bool split = top_p_mix && fused_sampler_enabled() != 0 && ws->can_fuse;
+  const bool fused = fused_sampler_enabled() != 0 && (!use_top_p || split) && ws->can_fuse;
+  if ((!fused || split) && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
   if (!use_graph || m->prof.on)
-    return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged, mixed_steps);
+    return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged, mixed_steps, split);
 
   const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
   CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
@@ -725,7 +751,7 @@ static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, 
   const int64_t* gz = ws->z_in.as<int64_t>();
   const int32_t* gmask = mask ? ws->mask_in.as<int32_t>() : nullptr;
   int64_t* gout = ws->z_out.as<int64_t>();
-  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged, mixed_steps};
+  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged, mixed_steps, split};
   auto it = ws->graphs.find(key);
   if (it == ws->graphs.end()) {
     cudaStream_t cap;
@@ -734,7 +760,7 @@ static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, 
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cap); return fail("begin capture: %s", cudaGetErrorString(e)); }
     const unsigned long long before = g_launches;
-    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged, mixed_steps);
+    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged, mixed_steps, split);
     const unsigned long long in_graph = g_launches - before;
     g_launches = before;
     e = cudaStreamEndCapture(cap, &graph);
@@ -770,10 +796,13 @@ int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask,
                          group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                           const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
-                           int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
-                           int32_t use_graph, int64_t* out, void* stream) {
+}  // extern "C"
+
+// vnb_generate_steps, and with mixed_top_p vnb_generate_mixed_top_p
+static int generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                          const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
+                          int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
+                          int32_t use_graph, int64_t* out, void* stream, bool mixed_top_p) {
   if (!group_steps || !group_gamma || !groups) return fail("vnb_generate_steps: group_steps, group_gamma and groups are required");
   if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
   for (int g = 0; g < n_groups; ++g) {
@@ -787,7 +816,25 @@ int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, 
     if (!group_gamma[g]) return fail("vnb_generate_steps: group %d lacks its schedules (gamma)", g);
   }
   return generate_launch(m, z, mask, B, T, group_steps[0], nullptr, group_steps, group_gamma, groups, n_groups,
-                         group_frames, group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream));
+                         group_frames, group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream), mixed_top_p);
+}
+
+extern "C" {
+
+int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                           const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
+                           int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
+                           int32_t use_graph, int64_t* out, void* stream) {
+  return generate_steps(m, z, mask, B, T, group_steps, group_gamma, groups, n_groups, group_frames, group_adapter,
+                        use_graph, out, stream, false);
+}
+
+int32_t vnb_generate_mixed_top_p(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                 const int32_t* group_steps, const float* const* group_gamma,
+                                 const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
+                                 const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
+  return generate_steps(m, z, mask, B, T, group_steps, group_gamma, groups, n_groups, group_frames, group_adapter,
+                        use_graph, out, stream, true);
 }
 
 // Calls of one length are the group_frames = NULL case.
@@ -1051,24 +1098,19 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
   CK(launch_gemm(p, st));
   return 0;
 }
-int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
-                       int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
-                       int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream) {
-  if (path < 0 || path > 3) return fail("vnb_dbg_sample: path %d outside 0..3", path);
-  if (B < 1 || T < 1 || ncc < 0 || C <= ncc) return fail("vnb_dbg_sample: need B >= 1, T >= 1 and 0 <= ncc < C");
-  if (V % 128 != 0 || V < 128 || V > 1024) return fail("vnb_dbg_sample: need V %% 128 == 0, 128 <= V <= 1024 (got %d)", V);
-  if (!zcur || !tokens || !conf || !n0 || !groups) return fail("vnb_dbg_sample: zcur, tokens, conf, n0 and groups are required");
-  if (path <= 1 && !logits) return fail("vnb_dbg_sample: path %d needs logits", path);
-  if (path == 2 && !partials) return fail("vnb_dbg_sample: path 2 needs partials");
-  if (n_groups < 1 || n_groups > B) return fail("vnb_dbg_sample: n_groups %d out of range 1..B (B = %d)", n_groups, B);
+}  // extern "C"
+
+// The [group] table of one step's sampling scalars and the row -> group map of B batch rows, built as
+// vnb_generate_many builds them and staged into dyn_dev / grp_dev (stream-ordered).
+static int stage_sample_groups(const vnb_sample_group* groups, int32_t n_groups, int32_t B, DevBuf& dyn_dev,
+                               DevBuf& grp_dev, cudaStream_t st, const char* who) {
+  if (n_groups < 1 || n_groups > B) return fail("%s: n_groups %d out of range 1..B (B = %d)", who, n_groups, B);
   long long total = 0;
   for (int g = 0; g < n_groups; ++g) {
-    if (groups[g].rows < 1) return fail("vnb_dbg_sample: group %d has %d rows", g, groups[g].rows);
+    if (groups[g].rows < 1) return fail("%s: group %d has %d rows", who, g, groups[g].rows);
     total += groups[g].rows;
   }
-  if (total != B) return fail("vnb_dbg_sample: group rows sum to %lld, not B = %d", total, B);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // one step's row of the [step][group] table and the row map, as vnb_generate_many_adapted fills them
+  if (total != B) return fail("%s: group rows sum to %lld, not B = %d", who, total, B);
   std::vector<SampleDyn> dyn(n_groups);
   std::vector<RowGroup> rowgrp(B);
   for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
@@ -1085,11 +1127,26 @@ int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, 
     d.top_p = q.top_p;
     for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
   }
-  DevBuf dyn_dev, grp_dev;
   CK(dyn_dev.alloc(sizeof(SampleDyn) * n_groups));
   CK(grp_dev.alloc(sizeof(RowGroup) * B));
   CK(cudaMemcpyAsync(dyn_dev.p, dyn.data(), sizeof(SampleDyn) * n_groups, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+// vnb_dbg_sample (paths 0..3) and vnb_dbg_sample_split (path 4: the split combine, the split nucleus draw, the re-mask)
+static int dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                      int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
+                      int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream,
+                      const char* who) {
+  if (B < 1 || T < 1 || ncc < 0 || C <= ncc) return fail("%s: need B >= 1, T >= 1 and 0 <= ncc < C", who);
+  if (V % 128 != 0 || V < 128 || V > 1024) return fail("%s: need V %% 128 == 0, 128 <= V <= 1024 (got %d)", who, V);
+  if (!zcur || !tokens || !conf || !n0 || !groups) return fail("%s: zcur, tokens, conf, n0 and groups are required", who);
+  if ((path <= 1 || path == 4) && !logits) return fail("%s: path %d needs logits", who, path);
+  if ((path == 2 || path == 4) && !partials) return fail("%s: path %d needs partials", who, path);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  DevBuf dyn_dev, grp_dev;
+  if (stage_sample_groups(groups, n_groups, B, dyn_dev, grp_dev, st, who)) return 1;
   SampleArgs sa;
   sa.logits = logits; sa.zcur = zcur; sa.zorig = zorig; sa.tokens = tokens; sa.conf = conf; sa.n0 = n0;
   sa.rowgrp = grp_dev.as<RowGroup>();
@@ -1098,7 +1155,55 @@ int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, 
   const SampleDyn* dd = dyn_dev.as<SampleDyn>();
   if (path <= 1) CK(launch_sample_step_dev(sa, dd, st, path == 1));
   else if (path == 2) CK(launch_sample_combine_dev(sa, partials, dd, st));
-  else CK(launch_remask_dev(sa, dd, st));
+  else if (path == 3) CK(launch_remask_dev(sa, dd, st));
+  else CK(launch_sample_split_dev(sa, partials, dd, st));
+  CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
+  return 0;
+}
+
+extern "C" {
+
+int32_t vnb_dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                       int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C, int32_t ncc,
+                       int32_t V, int32_t mask_token, const vnb_sample_group* groups, int32_t n_groups, void* stream) {
+  if (path < 0 || path > 3) return fail("vnb_dbg_sample: path %d outside 0..3", path);
+  return dbg_sample(path, logits, partials, zcur, zorig, tokens, conf, n0, B, T, C, ncc, V, mask_token, groups,
+                    n_groups, stream, "vnb_dbg_sample");
+}
+
+int32_t vnb_dbg_sample_split(const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
+                             int32_t* tokens, float* conf, const int32_t* n0, int32_t B, int32_t T, int32_t C,
+                             int32_t ncc, int32_t V, int32_t mask_token, const vnb_sample_group* groups,
+                             int32_t n_groups, void* stream) {
+  return dbg_sample(4, logits, partials, zcur, zorig, tokens, conf, n0, B, T, C, ncc, V, mask_token, groups, n_groups,
+                    stream, "vnb_dbg_sample_split");
+}
+
+int32_t vnb_dbg_gemm_sample_split(const void* A, const void* W, const float* bias, int32_t M, int32_t N, int32_t K,
+                                  const float* ss_in, int32_t ss_parts, float inv_d, float eps, const int32_t* zcur,
+                                  int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token,
+                                  const vnb_sample_group* groups, int32_t n_groups, void* partials, float* logits,
+                                  void* stream) {
+  if (V % 128 != 0 || V > 1024 || ncc < 0 || C <= ncc || N != (C - ncc) * V || T < 1 || M % T != 0)
+    return fail("vnb_dbg_gemm_sample_split: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1 "
+                "and M a multiple of T");
+  if (!bias || !zcur || !partials || !logits || !groups)
+    return fail("vnb_dbg_gemm_sample_split: bias, zcur, partials, logits and groups are required");
+  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_sample_split: ss_parts must be >= 1");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  DevBuf dyn_dev, grp_dev;
+  if (stage_sample_groups(groups, n_groups, M / T, dyn_dev, grp_dev, st, "vnb_dbg_gemm_sample_split")) return 1;
+  GemmPlan p;
+  if (!make_gemm_plan(&p, VNB_EPI_SAMPLE, A, W, M, N, K, nullptr, nullptr, bias, T, T, 0))
+    return fail("gemm plan: %s", tmap_error());
+  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
+  p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
+  p.dyn = dyn_dev.as<SampleDyn>();
+  p.rowgrp = grp_dev.as<RowGroup>();
+  p.out = logits;
+  p.sample_split = true;
+  p.live = g_dbg_live;
+  CK(launch_gemm(p, st));
   CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
   return 0;
 }

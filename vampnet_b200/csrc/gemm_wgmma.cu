@@ -305,7 +305,8 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[128], uint8_t* ring, 
 // element sees the same operands in the same K order as in the single-CTA variant: the two are bit-identical.  On an
 // H100 the single-CTA kernel is faster (the pair couples the two CTAs' progress and constrains their placement; same-
 // box A/B at the default bench workload: 403 vs 333 TFLOP/s for the GEMM family), so it is the default.
-template <int EPI, bool PAIR, bool ADAPT = false>
+// SPLIT (EPI_SAMPLE only): a launch that mixes nucleus (top-p) and plain groups; see the sampling epilogue.
+template <int EPI, bool PAIR, bool ADAPT = false, bool SPLIT = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmArgs g) {
@@ -436,7 +437,32 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int col0 = n0 + strip * 128;
         const int cp = col0 / g.V, v0 = col0 - cp * g.V;
         const int Cp = g.C - g.ncc;
-        const bool active = row_ok && __ldg(g.zcur + static_cast<size_t>(row) * g.C + g.ncc + cp) == g.mask_token;
+        bool active = row_ok && __ldg(g.zcur + static_cast<size_t>(row) * g.C + g.ncc + cp) == g.mask_token;
+        if constexpr (SPLIT) {
+          // A launch of nucleus (top-p) and plain groups: a still-masked position of a nucleus group gets no record.
+          // Its strip of logits goes to g.out instead, at the index and with the arithmetic of the materialising
+          // epilogue (drain_f32: acc * row scale, + bias), for sample_rows_kernel.  The warp stores one such row at a
+          // time, each lane four columns 32 apart: every store instruction is one contiguous 128-byte segment.
+          if (__any_sync(0xffffffffu, active)) {
+            const SampleDyn& dyn = g.dyn[g.rowgrp[row_ok ? b_idx : 0].group];
+            const bool nucleus = dyn.top_p > 0.f && dyn.top_p < 1.f;
+            uint32_t pend = __ballot_sync(0xffffffffu, active && nucleus);
+            float* const strip_out = reinterpret_cast<float*>(g.out) + static_cast<size_t>(row_base) * g.N + col0 + lane;
+            const uint32_t src = qaddr + 4u * (strip * 128 + lane);
+            const uint32_t bsrc = sbias + 4u * (strip * 128 + lane);
+            while (pend != 0u) {
+              const int r = __ffs(pend) - 1;
+              pend &= pend - 1u;
+              const float rsr = __shfl_sync(0xffffffffu, rs, r);
+              float* const dst = strip_out + static_cast<size_t>(r) * g.N;
+#pragma unroll
+              for (int k = 0; k < 4; ++k)
+                dst[32 * k] = __fadd_rn(__fmul_rn(lds_f32(src + 4u * (r * ACC_PITCH + 32 * k)), rsr),
+                                        lds_f32(bsrc + 128u * k));
+            }
+            active = active && !nucleus;
+          }
+        }
         if (__any_sync(0xffffffffu, active)) {
           const uint32_t t_strip = t_addr + 4u * (strip * 128);
           const uint32_t sb4 = sbias + 4u * (strip * 128);
@@ -758,6 +784,14 @@ static cudaError_t init_epi() {
     e = cudaFuncSetAttribute(gemm_geglu_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GG_SMEM);
     if (e != cudaSuccess) return e;
   }
+  if constexpr (EPI == VNB_EPI_SAMPLE) {
+    e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             GEMM_SMEM);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             GEMM_SMEM);
+    if (e != cudaSuccess) return e;
+  }
   cudaLaunchConfig_t q = {};
   q.gridDim = dim3(2 * device_sm_count());
   q.blockDim = dim3(GEMM_THREADS);
@@ -793,7 +827,7 @@ int get_gemm_max_clusters() {
 // One CTA per output tile (the accumulator tile overlays the operand ring, so a CTA does not start a second tile), except
 // for the FFN-up GEMM without adapters: the persistent kernel, one CTA per SM (the SM count is cached by prepare_gemm(),
 // so none is queried inside a capture).
-template <int EPI, bool ADAPT = false>
+template <int EPI, bool ADAPT = false, bool SPLIT = false>
 static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t st) {
   cudaError_t e = init_epi<EPI>();
   if (e != cudaSuccess) return e;
@@ -808,7 +842,7 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true, ADAPT>, p.tmA, p.tmBh, g);
+    return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true, ADAPT, SPLIT>, p.tmA, p.tmBh, g);
   }
   const int tiles = ((g.M + BM - 1) / BM) * (g.N / BN);
   if constexpr (EPI == VNB_EPI_GEGLU && !ADAPT) {
@@ -816,7 +850,7 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
     gemm_geglu_persistent_kernel<<<grid, GG_THREADS, GG_SMEM, st>>>(p.tmA, p.tmB, g);
     return cudaGetLastError();
   }
-  gemm_wgmma_kernel<EPI, false, ADAPT><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
+  gemm_wgmma_kernel<EPI, false, ADAPT, SPLIT><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
   return cudaGetLastError();
 }
 
@@ -848,6 +882,10 @@ cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
     case VNB_EPI_BIAS_F32: return launch_epi<VNB_EPI_BIAS_F32>(p, g, st);
     case VNB_EPI_SAMPLE:
       if (!p.zcur || !p.dyn || !p.rowgrp || !p.partials || !p.bias || p.V % 128 != 0 || p.V > 1024) return cudaErrorInvalidValue;
+      if (p.sample_split) {
+        if (!p.out) return cudaErrorInvalidValue;
+        return launch_epi<VNB_EPI_SAMPLE, false, true>(p, g, st);
+      }
       return launch_epi<VNB_EPI_SAMPLE>(p, g, st);
     default: return cudaErrorInvalidValue;
   }

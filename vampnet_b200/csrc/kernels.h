@@ -92,6 +92,9 @@ struct GemmPlan {
   const SampleDyn* dyn = nullptr;    // this step's scalars, one per group (device memory: graph replay safe)
   const RowGroup* rowgrp = nullptr;  // (B) group of every batch row
   void* partials = nullptr;          // (M * Cp * V/128) float4 records, see sample_combine_kernel
+  // a launch of nucleus (top-p) and plain groups: the rows of nucleus groups store their logits to `out` (the
+  // materialising epilogue's layout, still-masked positions only) and leave no records
+  bool sample_split = false;
   int C = 0, ncc = 0, V = 0, mask_token = 0;
   // adapted variant of QKV / RESID / GEGLU (null table: the plain kernel): acc += u[row] . B'[col] for adapted rows
   AdapterRefs lora;
@@ -171,8 +174,11 @@ struct SampleArgs {
 cudaError_t launch_sample_step_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st, bool use_top_p);
 // fused path: the classifier's sampling epilogue wrote `partials`; picks the tile, writes tokens + confidences, re-masks
 cudaError_t launch_sample_combine_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
-// the re-mask alone (the second kernel of both launchers above): reads a.tokens and a.conf, updates a.zcur
+// the re-mask alone (the second kernel of the launchers): reads a.tokens and a.conf, updates a.zcur
 cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cudaStream_t st);
+// a launch of nucleus (top-p) and plain groups after the split classifier epilogue: the combine serves the rows of plain
+// groups from `partials`, the nucleus draw the rows of top-p groups from a.logits, then the re-mask
+cudaError_t launch_sample_split_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
 
 // ---- onset detection (onset.cu; librosa 0.10 onset_detect restated, DESIGN.md §9) ----
 // peak_pick windows of onset_detect's defaults at (sr, hop), and the envelope's left padding lag + n_fft // (2 hop)

@@ -15,6 +15,9 @@
 //                          lane, float4), warp-shuffle max / sum-exp, the same two-level inverse-CDF draw with two
 //                          counter-based Philox uniforms per row, writes token + confidence.  Known positions cost
 //                          4 bytes.  Algorithmic bytes: V*4 per masked position.
+// A fused launch that mixes nucleus and plain groups runs both draws after the split classifier epilogue, each kernel
+// on its own groups' rows only: sample_combine_kernel<true> from the records, sample_rows_kernel<true, true> from the
+// logits the epilogue stored for the nucleus rows; then remask_kernel.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -41,8 +44,10 @@ struct SampleStatic {
   const int32_t* live;  // (1) batch rows b >= live[0] are idle this iteration and left untouched; null: all live
 };
 
-// TOPP = false compiles the nucleus filter out (its 32 extra live registers cost occupancy on the common path)
-template <bool TOPP>
+// TOPP = false compiles the nucleus filter out (its 32 extra live registers cost occupancy on the common path).
+// SPLIT (with TOPP): a launch of nucleus and plain groups; this kernel serves the rows of nucleus groups only and leaves
+// the others to sample_combine_kernel<true>.
+template <bool TOPP, bool SPLIT = false>
 __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const SampleStatic a, const SampleDynDev* __restrict__ dynp) {
   const int Cp = a.C - a.ncc;
   const int S = a.T * Cp;
@@ -53,6 +58,9 @@ __global__ void __launch_bounds__(256, TOPP ? 2 : 3) sample_rows_kernel(const Sa
   if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle call's row: its state is not touched
   const RowGroup rg = a.rowgrp[b];
   const SampleDynDev dyn = dynp[rg.group];
+  if constexpr (SPLIT) {
+    if (!(dyn.top_p > 0.f && dyn.top_p < 1.f)) return;  // a plain group's row: not touched
+  }
   const uint32_t bg = static_cast<uint32_t>(b - rg.first);  // Philox counter word: the row within its own call
   const int t = s / Cp, cp = s - t * Cp;
   const int zi = a.zcur[(static_cast<size_t>(b) * a.T + t) * a.C + a.ncc + cp];
@@ -339,6 +347,8 @@ __global__ void __launch_bounds__(1024) remask_kernel(const SampleStatic a, cons
 // with uniform 2.  One thread per row: pick the tile with uniform 1 by mass, take its candidate, and compute
 // confidence = log softmax(token) + temperature * Gumbel exactly as sample_rows_kernel does.  The logits themselves
 // never reach HBM.  Algorithmic bytes: 16 * V/128 per masked row.
+// SPLIT: a launch of nucleus and plain groups; the rows of nucleus groups are left to sample_rows_kernel<true, true>.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic a, const float4* __restrict__ partials,
                                                              const SampleDynDev* __restrict__ dynp) {
   const int Cp = a.C - a.ncc;
@@ -349,6 +359,9 @@ __global__ void __launch_bounds__(256) sample_combine_kernel(const SampleStatic 
   if (a.live != nullptr && b >= __ldg(a.live)) return;  // an idle call's row: tokens and confidences are not touched
   const RowGroup rg = a.rowgrp[b];
   const SampleDynDev dyn = dynp[rg.group];
+  if constexpr (SPLIT) {
+    if (dyn.top_p > 0.f && dyn.top_p < 1.f) return;  // a nucleus group's row: not touched
+  }
   const uint32_t bg = static_cast<uint32_t>(b - rg.first);
   const int t = s / Cp, cp = s - t * Cp;
   const int zi = a.zcur[(static_cast<size_t>(b) * a.T + t) * a.C + a.ncc + cp];
@@ -437,8 +450,21 @@ cudaError_t launch_sample_combine_dev(const SampleArgs& s, const void* partials,
   const SampleStatic a = make_static(s);
   if (s.V % 128 != 0 || s.V > 1024) return cudaErrorInvalidValue;
   const int rows = s.B * s.T * (s.C - s.ncc);
-  sample_combine_kernel<<<(rows + 255) / 256, 256, 0, st>>>(a, reinterpret_cast<const float4*>(partials), dyn_dev);
+  sample_combine_kernel<false><<<(rows + 255) / 256, 256, 0, st>>>(a, reinterpret_cast<const float4*>(partials), dyn_dev);
   cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return launch_remask_dev(s, dyn_dev, st);
+}
+
+cudaError_t launch_sample_split_dev(const SampleArgs& s, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st) {
+  const SampleStatic a = make_static(s);
+  if (s.V % 128 != 0 || s.V > 1024) return cudaErrorInvalidValue;
+  const int rows = s.B * s.T * (s.C - s.ncc);
+  sample_combine_kernel<true><<<(rows + 255) / 256, 256, 0, st>>>(a, reinterpret_cast<const float4*>(partials), dyn_dev);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  sample_rows_kernel<true, true><<<(rows + 7) / 8, 256, 0, st>>>(a, dyn_dev);
+  e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   return launch_remask_dev(s, dyn_dev, st);
 }

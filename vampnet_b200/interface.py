@@ -364,7 +364,8 @@ class Interface(torch.nn.Module):
         return self._vamp_result(z, zv, coarse_start, fine_start, return_mask)
 
     @torch.inference_mode()
-    def vamp_many(self, requests: list, mixed_lengths: bool = False, mixed_steps: bool = False):
+    def vamp_many(self, requests: list, mixed_lengths: bool = False, mixed_steps: bool = False,
+                  mixed_top_p: bool = False):
         """Serve many vamp() calls together.  Each request is a dict of vamp() arguments (codes, mask, and optionally
         batch_size, feedback_steps, time_stretch_factor, return_mask and generate keyword arguments).  Returns the
         list the sequential vamp() calls return, bit for bit, and leaves the random, numpy and torch RNG states as
@@ -378,11 +379,16 @@ class Interface(torch.nn.Module):
         stages), so a request's remainder chunk need not run in a launch of its own; the results are the same.
 
         mixed_steps=True: chunks of requests with different sampling-step counts share launches too
-        (generate_many(mixed_steps=True) in both stages); the results are the same."""
+        (generate_many(mixed_steps=True) in both stages); the results are the same.
+
+        mixed_top_p=True: chunks of nucleus (top-p) and plain-sampling requests share launches too
+        (generate_many(mixed_top_p=True) in both stages); the results are the same."""
         from .modules.transformer import draw_philox_key
         many = dict(mixed_lengths=True) if mixed_lengths else {}
         if mixed_steps:
             many["mixed_steps"] = True
+        if mixed_top_p:
+            many["mixed_top_p"] = True
         reqs = []
         for r in requests:
             r = dict(r)

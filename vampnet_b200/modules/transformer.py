@@ -671,7 +671,8 @@ class VampNet(nn.Module):
         return out
 
     @torch.inference_mode()
-    def generate_many(self, codec, calls, mixed_lengths: bool = False, mixed_steps: bool = False):
+    def generate_many(self, codec, calls, mixed_lengths: bool = False, mixed_steps: bool = False,
+                      mixed_top_p: bool = False):
         """Run many independent generate() calls, batched into as few launches as the shapes allow.
 
         `calls` is a list of dicts of generate() keyword arguments.  The result equals
@@ -688,7 +689,11 @@ class VampNet(nn.Module):
         mixed_steps=True: calls of different sampling-step counts share launches too (vnb_generate_steps; the bucket key
         drops the steps, the MANY_MAX_ROWS split is unchanged).  Each launch's calls are ordered by steps, longest first
         (stable); a launch runs as many iterations as its longest call, and a call of fewer steps is idle, and costs
-        close to nothing, until its own steps fill the launch's last iterations.  The results are still bit-identical."""
+        close to nothing, until its own steps fill the launch's last iterations.  The results are still bit-identical.
+
+        mixed_top_p=True: nucleus (top-p) and plain-sampling calls share launches too (vnb_generate_mixed_top_p; the
+        bucket key drops top-p on/off, the MANY_MAX_ROWS split and the orders above are unchanged).  Each row draws as
+        its own call would; the results are still bit-identical."""
         import inspect
         sig = inspect.signature(VampNet.generate)
         prepared, want_signal = [], []
@@ -701,7 +706,7 @@ class VampNet(nn.Module):
                                                a["ctrl_masks"], a["top_p"], a["seed"], a["sample_cutoff"],
                                                a["cfg_guidance"], a["philox_key"], a["adapter"]))
             want_signal.append(bool(a["return_signal"]))
-        outs = self._launch_calls(prepared, mixed_lengths, mixed_steps)
+        outs = self._launch_calls(prepared, mixed_lengths, mixed_steps, mixed_top_p)
         return [self.decode(o, codec) if sig_ else o for o, sig_ in zip(outs, want_signal)]
 
     def _prepare_call(self, codec, time_steps, steps, start_tokens, temperature, mask, mask_temperature, ctrls,
@@ -741,16 +746,18 @@ class VampNet(nn.Module):
                     do_sample=[1 if (i / steps) <= sample_cutoff else 0 for i in range(steps)], key=k,
                     top_p=float(top_p) if (top_p is not None and top_p < 1.0) else 0.0, adapter=adapter)
 
-    def _launch_calls(self, calls: list, mixed_lengths: bool = False, mixed_steps: bool = False) -> list:
+    def _launch_calls(self, calls: list, mixed_lengths: bool = False, mixed_steps: bool = False,
+                      mixed_top_p: bool = False) -> list:
         """Launch prepared calls, one vnb_generate_many per (T, steps, top-p on) bucket of at most MANY_MAX_ROWS rows
         (a single larger call runs alone); returns each call's (B, C, T) int64 tokens in list order.
         mixed_lengths: buckets drop T; a bucket's calls, longest first, fill launches while rows * (the launch's longest
         T) stays within MANY_MAX_ROWS.
         mixed_steps: buckets drop the steps; each launch's calls are then ordered by steps, longest first (stable), as
-        vnb_generate_steps requires."""
+        vnb_generate_steps requires.
+        mixed_top_p: buckets drop top-p on/off."""
         buckets = {}
         for i, c in enumerate(calls):
-            top_p_on = 0.0 < c["top_p"] < 1.0
+            top_p_on = None if mixed_top_p else 0.0 < c["top_p"] < 1.0
             T = None if mixed_lengths else c["z"].shape[-1]
             buckets.setdefault((T, None if mixed_steps else c["steps"], top_p_on), []).append(i)
         launches = []
@@ -817,11 +824,12 @@ class VampNet(nn.Module):
     def _launch(self, calls: list, keep: list, z, m32, frames=None):
         """One launch of the prepared calls on their concatenated (B, C, T) z / mask; frames: each call's own length
         (vnb_generate_ragged), None when all have T.  Calls of different step counts (longest first) launch through
-        vnb_generate_steps."""
+        vnb_generate_steps, nucleus (top-p) calls next to plain ones through vnb_generate_mixed_top_p."""
         dev = self.device
         B, _, T = z.shape
         steps = calls[0]["steps"]
         mixed_steps = any(c["steps"] != steps for c in calls)
+        mixed_top_p = len({0.0 < c["top_p"] < 1.0 for c in calls}) > 1
         arrays = []
         groups = (_lib.GenGroup * len(calls))()
         for g, c in zip(groups, calls):
@@ -836,14 +844,14 @@ class VampNet(nn.Module):
         out = torch.empty_like(z)
         graph = 1 if self.use_cuda_graph else 0
         with torch.cuda.device(dev):
-            if mixed_steps:
+            if mixed_steps or mixed_top_p:
                 gams = [(C.c_float * c["steps"])(*c["gamma"]) for c in calls]
                 gptr = (C.POINTER(C.c_float) * len(calls))(*[C.cast(a, C.POINTER(C.c_float)) for a in gams])
                 fr = None if frames is None else (C.c_int32 * len(calls))(*frames)
-                _lib.check(_lib.lib().vnb_generate_steps(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T,
-                                                         (C.c_int32 * len(calls))(*[c["steps"] for c in calls]), gptr,
-                                                         groups, len(calls), fr, ids, graph, _lib.ptr(out),
-                                                         _lib.stream_ptr(dev)))
+                fn = _lib.lib().vnb_generate_mixed_top_p if mixed_top_p else _lib.lib().vnb_generate_steps
+                _lib.check(fn(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T,
+                              (C.c_int32 * len(calls))(*[c["steps"] for c in calls]), gptr, groups, len(calls), fr, ids,
+                              graph, _lib.ptr(out), _lib.stream_ptr(dev)))
             elif frames is not None:
                 _lib.check(_lib.lib().vnb_generate_ragged(self._handle, _lib.ptr(z), _lib.ptr(m32), B, T, steps, gam,
                                                           groups, len(calls), (C.c_int32 * len(calls))(*frames), ids,
