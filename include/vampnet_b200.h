@@ -278,12 +278,15 @@ enum {
 int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
                     void* out2, const float* bias, int32_t T, int32_t Tpad, void* stream);
 /* Fused self-attention with relative-position bias (transformer.py:234-254).
- * qk (B, T, 2d) bf16 [q | k], vT (B, d, Tpad) bf16, out (B, T, d) bf16, d = H*64. */
+ * qk (B, T, 2d) bf16 [q | k], vT (B, d, Tpad) bf16, out (B, T, d) bf16, d = H*64; rel_bias (2*rel_sat+1, H) fp32 with
+ * entry [clamp(k - q, -rel_sat, rel_sat) + rel_sat, h].  Preconditions: rel_sat in 1..128, Tpad >= T and a multiple of
+ * 8 (refused otherwise), every table entry finite, and the v^T padding columns [T, Tpad) finite (the mask gives them
+ * weight 0, and 0 * inf would be NaN). */
 int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                          int32_t B, int32_t T, int32_t Tpad, int32_t H, void* stream);
 /* Test-only: vnb_op_attention with a key length per batch row, frames DEVICE [B], entries in 1..T.  Row b attends to
  * keys t < frames[b] only and writes out rows t < frames[b] only; its later rows of qk may hold anything, its later
- * columns of vT must be zero (as the QKV epilogue of vnb_dbg_gemm_qkv_frames leaves them).  Query tiles wholly past
+ * columns of vT must be finite (the QKV epilogue of vnb_dbg_gemm_qkv_frames leaves them zero).  Query tiles wholly past
  * frames[b] do no work. */
 int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                                  int32_t B, int32_t T, int32_t Tpad, int32_t H, const int32_t* frames, void* stream);

@@ -952,6 +952,7 @@ int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_
 }
 int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat, int32_t B,
                          int32_t T, int32_t Tpad, int32_t H, void* stream) {
+  if (T < 1 || Tpad < T) return fail("vnb_op_attention: need 1 <= T <= Tpad");
   AttnPlan p;
   if (!make_attn_plan(&p, qk, vT, out, rel_bias, rel_sat, B, T, Tpad, H)) return fail("attn plan: %s", tmap_error());
   p.live = g_dbg_live;
@@ -961,6 +962,7 @@ int32_t vnb_op_attention(const void* qk, const void* vT, void* out, const float*
 int32_t vnb_dbg_attention_ragged(const void* qk, const void* vT, void* out, const float* rel_bias, int32_t rel_sat,
                                  int32_t B, int32_t T, int32_t Tpad, int32_t H, const int32_t* frames, void* stream) {
   if (!frames) return fail("vnb_dbg_attention_ragged: frames is required");
+  if (T < 1 || Tpad < T) return fail("vnb_dbg_attention_ragged: need 1 <= T <= Tpad");
   AttnPlan p;
   if (!make_attn_plan(&p, qk, vT, out, rel_bias, rel_sat, B, T, Tpad, H)) return fail("attn plan: %s", tmap_error());
   p.frames = frames;

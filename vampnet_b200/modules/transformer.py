@@ -162,6 +162,18 @@ def relative_position_bucket(rel: torch.Tensor, num_buckets: int = 32, max_dista
     return ret + torch.where(n < exact, n, big)
 
 
+def rel_bias_table(weight: torch.Tensor):
+    """The attention kernel's bias operand from the per-bucket weights (32, H): the Toeplitz table (2*sat+1, H) fp32
+    over key - query in [-sat, sat], and sat, the distance beyond which the bucket no longer changes (91 for the
+    reference's 32 buckets / max_distance 128), found from the bucket function itself."""
+    probe = relative_position_bucket(torch.arange(-REL_SAT, REL_SAT + 1))
+    sat = REL_SAT
+    while sat > 1 and probe[REL_SAT + sat - 1] == probe[-1] and probe[REL_SAT - (sat - 1)] == probe[0]:
+        sat -= 1
+    buckets = relative_position_bucket(torch.arange(-sat, sat + 1)).to(weight.device)
+    return weight.float()[buckets].contiguous(), sat
+
+
 def gamma_schedule(steps: int):
     """Per-step fp32 schedule values computed exactly as the reference does on CPU
     (util.py:6-7 -> fp32 tensor; mask.py:8-9; transformer.py:831-834, 917-919)."""
@@ -524,16 +536,7 @@ class VampNet(nn.Module):
         # channel r = p*Cp + c  ->  row c*V + p, so a row-major (M, Cp*V) store IS (B, S = t*Cp + c, V)
         p["wcls"] = w.view(V, Cp, d).permute(1, 0, 2).reshape(Cp * V, d).to(bf).contiguous()
         p["bcls"] = wn.bias.float().view(V, Cp).t().reshape(-1).contiguous()
-        # Toeplitz bias table over key-query in [-sat, sat]; sat = the distance beyond which the bucket no longer
-        # changes (91 for the reference's 32 buckets / max_distance 128), found from the bucket function itself
-        probe = relative_position_bucket(torch.arange(-REL_SAT, REL_SAT + 1))
-        sat = REL_SAT
-        while sat > 1 and probe[REL_SAT + sat - 1] == probe[-1] and probe[REL_SAT - (sat - 1)] == probe[0]:
-            sat -= 1
-        self._rel_sat = sat
-        rel = torch.arange(-sat, sat + 1)
-        buckets = relative_position_bucket(rel).to(dev)
-        p["rel_bias"] = lay[0].self_attn.relative_attention_bias.weight.float()[buckets].contiguous()  # (2*sat+1, H)
+        p["rel_bias"], self._rel_sat = rel_bias_table(lay[0].self_attn.relative_attention_bias.weight.to(dev))
         return p
 
     def _ensure_handle(self, codec):
