@@ -221,6 +221,11 @@ __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ uint2 lds_u2(uint32_t addr) {
+  uint2 v;
+  asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+  return v;
+}
 __device__ __forceinline__ void sts_f4(uint32_t addr, float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
                : "memory");

@@ -15,8 +15,8 @@
 //                accumulators per thread; then the epilogue: the accumulators go to a padded fp32 tile that overlays the
 //                drained ring, and each epilogue warp reads 32 x 32 chunks of it in store order -> fused op -> global
 //                (4 warps; 8 for the residual and the sampling epilogues)
-// The FFN-up GEMM without adapters runs gemm_geglu_persistent_kernel instead: the same mainloop in one CTA per SM, with
-// each tile's stores overlapping the next tile's MMAs.
+// The FFN-up and QKV GEMMs without adapters run gemm_persistent_kernel instead: the same mainloop in one CTA per SM,
+// with each tile's stores overlapping the next tile's MMAs.
 //
 // Roofline: tensor-bound.  Algorithmic work = 2*M*N*K flop per launch; bytes (A+W+out) are a few
 // MB against > 10 GFLOP, far right of the ridge.
@@ -272,10 +272,10 @@ __device__ __forceinline__ void lora_update(const GemmArgs& g, uint8_t* scratch,
 }
 
 // The k-block loop of one tile (consumer warpgroup `wg`, rows [64 wg, 64 wg + 64)): acc += A W^T over every k-block in
-// order, 4 x k16 per 64-wide k-block.  `stage` / `phase` are the ring position of the first k-block and are left at
-// the one after the last, so a persistent CTA continues the ring from tile to tile.  release(s) hands stage s back to
-// the producer once the MMAs reading it have retired.
-template <typename Release>
+// order, 4 x k16 per 64-wide k-block, from a ring of NS stages.  `stage` / `phase` are the ring position of the first
+// k-block and are left at the one after the last, so a persistent CTA continues the ring from tile to tile.  release(s)
+// hands stage s back to the producer once the MMAs reading it have retired.
+template <int NS, typename Release>
 __device__ __forceinline__ void gemm_mainloop(float (&acc)[128], uint8_t* ring, uint64_t* full_bar, int num_kb, int wg,
                                               int& stage, uint32_t& phase, Release&& release) {
 #pragma unroll
@@ -291,12 +291,12 @@ __device__ __forceinline__ void gemm_mainloop(float (&acc)[128], uint8_t* ring, 
     wgmma_commit();
     wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
     wgmma_fence_regs(acc);
-    if (kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
-    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    if (kb > 0) release(stage == 0 ? NS - 1 : stage - 1);
+    if (++stage == NS) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
-  if (num_kb > 0) release(stage == 0 ? STAGES - 1 : stage - 1);
+  if (num_kb > 0) release(stage == 0 ? NS - 1 : stage - 1);
 }
 
 // PAIR = true: clusters of two CTAs on vertically adjacent 128 x 256 tiles (the same 256 W rows).  Each CTA fetches
@@ -372,7 +372,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const uint32_t peer_empty = PAIR ? mapa_u32(smem_u32(empty_bar), rank ^ 1u) : 0u;
       int stage = 0;
       uint32_t phase = 0;
-      gemm_mainloop(acc, smem, full_bar, num_kb, wg, stage, phase, [&](int s) {
+      gemm_mainloop<STAGES>(acc, smem, full_bar, num_kb, wg, stage, phase, [&](int s) {
         if (lane == 0) {
           mbar_arrive(&empty_bar[s]);
           if constexpr (PAIR) mbar_arrive_cluster(peer_empty + 8u * s);
@@ -612,42 +612,60 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if constexpr (PAIR) cluster_sync_all();
 }
 
-// Persistent FFN-up GEMM (GEGLU, no adapters): one CTA per SM walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ...
-// in the same n-fastest order, and a tile's stores run on dedicated warps while the consumers compute the next tile.
-//   warp 11      TMA producer: the same 4-stage ring as gemm_wgmma_kernel, continued across tile boundaries
-//   warps 0..7   consumers: the same mainloop; then value * gelu_tanh(gate) in registers (value column c and gate column
-//                c + 128 are fragments i and i + 16 of the same thread), rounded to bf16 into the staging tile
-//   warps 8..10  epilogue: copy the staging tile to global memory in whole rows, then compute the row scales of the
-//                CTA's next tile into shared memory
-// Handing over only the 128 x 128 bf16 result (32 KiB) leaves room for the full ring.  Per output element the operands,
-// the k order, the accumulator and the arithmetic (row scale, GEGLU, rounding) are those of gemm_wgmma_kernel's GEGLU
-// epilogue: bit-identical.
-constexpr int GG_EPI_WARPS = 3;
-constexpr int GG_THREADS = 256 + 32 * GG_EPI_WARPS + 32;  // 384: ptxas sizes registers per SM sub-partition, a 13th
-                                                          // warp would cap every thread at 128
-constexpr int GG_STAGE_BYTES = BM * (BN / 2) * 2;  // bf16 result tile, rows of 256 B, 16-byte units XOR-swizzled by row
-constexpr int GG_SMEM = RING_BYTES + GG_STAGE_BYTES + 4 * BM /*row scales*/ + 1024 /*align slack*/ + 128 /*barriers*/;
-static_assert(GG_SMEM <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
+// Persistent layer GEMMs without adapters, FFN-up (GEGLU) and QKV: one CTA per SM walks the tiles blockIdx.x,
+// blockIdx.x + gridDim.x, ... in the same n-fastest order, and a tile's stores run on dedicated warps while the
+// consumers compute the next tile.
+//   warp 11      TMA producer: a ring of {A 128x64, W 256x64} stages as in gemm_wgmma_kernel, continued across tile
+//                boundaries (GEGLU: 4 stages; QKV: 3, its staging tile is twice as large)
+//   warps 0..7   consumers: the same mainloop; then the row scale (and GEGLU) in registers, rounded to bf16 into the
+//                staging tile
+//   warps 8..10  epilogue: copy the staging tile to global memory, then compute the row scales of the CTA's next tile
+//                into shared memory
+// GEGLU: value * gelu_tanh(gate) (value column c and gate column c + 128 are fragments i and i + 16 of the same thread),
+// a 128 x 128 result stored in whole rows.  QKV: every 256-column tile is wholly q / k or wholly v (N = 3 d and
+// N % 256 == 0, so d2 = 2 d is a multiple of 512); q / k tiles are staged row-major and stored in whole rows at pitch
+// d2, v tiles are staged transposed and stored as runs of t into v^T (B, d, Tpad).
+// Per output element the operands, the k order, the accumulator and the arithmetic (row scale, GEGLU, rounding, the
+// frames select) are those of gemm_wgmma_kernel's epilogue: bit-identical.
+constexpr int PERS_EPI_WARPS = 3;
+constexpr int PERS_THREADS = 256 + 32 * PERS_EPI_WARPS + 32;  // 384: ptxas sizes registers per SM sub-partition, a
+                                                              // 13th warp would cap every thread at 128
+template <int EPI> constexpr int pers_stages() { return EPI == VNB_EPI_QKV ? 3 : STAGES; }
+// bf16 result tile: GEGLU 128 x 128 (rows of 256 B), QKV 128 x 256 (q / k: rows of 512 B; v: 256 d-rows of 256 B)
+template <int EPI> constexpr int pers_out_bytes() { return EPI == VNB_EPI_QKV ? BM * BN * 2 : BM * (BN / 2) * 2; }
+template <int EPI>
+constexpr int pers_smem() {
+  return pers_stages<EPI>() * STAGE_BYTES + pers_out_bytes<EPI>() + 4 * BM /*row scales*/ + 1024 /*align slack*/ +
+         128 /*barriers*/;
+}
+static_assert(pers_smem<VNB_EPI_GEGLU>() <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
+static_assert(pers_smem<VNB_EPI_QKV>() <= 227 * 1024, "H100: at most 227 KiB of shared memory per block");
 static_assert((2 * STAGES + 2) * 8 <= 128, "the barriers fit their slot");
 
-// byte offset of the 4-byte word holding result columns (2 w, 2 w + 1) of tile row r in the staging tile: the 16-byte
-// unit w / 4 is XORed with r % 8, so the consumers' fragment stores (8 rows x 4 words) and the epilogue's row reads
-// (8 consecutive units of one row) are both bank-conflict free
-__device__ __forceinline__ uint32_t gg_stage_off(int r, int w) {
-  return static_cast<uint32_t>(r * 256 + (((w >> 2) ^ (r & 7)) << 4) + ((w & 3) << 2));
+// byte offset of the 4-byte word w of row r in a staging tile of PITCH-byte rows: the 16-byte unit w / 4 is XORed with
+// r % 8, so the consumers' fragment stores (8 rows x 4 words) and the epilogue's row reads (consecutive units of one
+// row) are both bank-conflict free.  The transposed v tile is the PITCH = 256 case with one row per d-row, word w
+// holding tile rows 2 w and 2 w + 1.
+template <int PITCH>
+__device__ __forceinline__ uint32_t stage_off(int r, int w) {
+  return static_cast<uint32_t>(r * PITCH + (((w >> 2) ^ (r & 7)) << 4) + ((w & 3) << 2));
 }
 
-__global__ void __launch_bounds__(GG_THREADS, 1)
-gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                             const GemmArgs g) {
+template <int EPI>
+__global__ void __launch_bounds__(PERS_THREADS, 1)
+gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const GemmArgs g) {
+  constexpr int NS = pers_stages<EPI>();
+  constexpr int RING = NS * STAGE_BYTES;
+  constexpr int OUT_BYTES = pers_out_bytes<EPI>();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t stage_tile = smem_u32(smem + RING_BYTES);
-  float* srs = reinterpret_cast<float*>(smem + RING_BYTES + GG_STAGE_BYTES);  // row scales of the tile being computed
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING_BYTES + GG_STAGE_BYTES + 4 * BM);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* out_full = empty_bar + STAGES;  // the staging tile holds a result tile (256 consumer threads)
-  uint64_t* out_free = out_full + 1;        // the staging tile is free and srs holds the next tile's row scales
+  const uint32_t stage_tile = smem_u32(smem + RING);
+  float* srs = reinterpret_cast<float*>(smem + RING + OUT_BYTES);  // row scales of the tile being computed
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RING + OUT_BYTES + 4 * BM);
+  uint64_t* empty_bar = full_bar + NS;
+  uint64_t* out_full = empty_bar + NS;  // the staging tile holds a result tile (256 consumer threads)
+  uint64_t* out_free = out_full + 1;    // the staging tile is free and srs holds the next tile's row scales
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -655,17 +673,17 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
   const int num_kb = g.K / BK;
   // m-major tile order: the tiles of the live rows are a prefix; every warp role reads the same bound
   const int tiles = ((live_rows(g) + BM - 1) / BM) * num_n;
-  constexpr int kProducer = 8 + GG_EPI_WARPS;
+  constexpr int kProducer = 8 + PERS_EPI_WARPS;
 
   if (warp == kProducer && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
+    for (int s = 0; s < NS; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);  // lane 0 of every consumer warp
     }
     mbar_init(out_full, 256);
-    mbar_init(out_free, 32 * GG_EPI_WARPS);
+    mbar_init(out_free, 32 * PERS_EPI_WARPS);
     mbar_fence_init();
   }
   __syncthreads();
@@ -683,7 +701,7 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
           mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
           tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m0);
           tma_load_2d(sa + A_BYTES, &tmB, &full_bar[stage], kb * BK, n0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (++stage == NS) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -697,23 +715,49 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
     const int r = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
       float acc[128];
-      gemm_mainloop(acc, smem, full_bar, num_kb, warp >> 2, stage, phase, [&](int s) {
+      gemm_mainloop<NS>(acc, smem, full_bar, num_kb, warp >> 2, stage, phase, [&](int s) {
         if (lane == 0) mbar_arrive(&empty_bar[s]);
       });
       mbar_wait(out_free, it & 1u);  // the previous result tile is stored, srs holds this tile's row scales
       const float rs0 = srs[r], rs1 = srs[r + 8];
+      if constexpr (EPI == VNB_EPI_GEGLU) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        float x[4];
+        for (int i = 0; i < 16; ++i) {
+          float x[4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float rsr = k < 2 ? rs0 : rs1;
-          x[k] = acc[4 * i + k] * rsr;
-          x[k] = x[k] * gelu_tanh(acc[4 * (i + 16) + k] * rsr);
+          for (int k = 0; k < 4; ++k) {
+            const float rsr = k < 2 ? rs0 : rs1;
+            x[k] = acc[4 * i + k] * rsr;
+            x[k] = x[k] * gelu_tanh(acc[4 * (i + 16) + k] * rsr);
+          }
+          const int w = 4 * i + (lane & 3);
+          sts_u32(stage_tile + stage_off<256>(r, w), pack_bf16x2(x[0], x[1]));
+          sts_u32(stage_tile + stage_off<256>(r + 8, w), pack_bf16x2(x[2], x[3]));
         }
-        const int w = 4 * i + (lane & 3);
-        sts_u32(stage_tile + gg_stage_off(r, w), pack_bf16x2(x[0], x[1]));
-        sts_u32(stage_tile + gg_stage_off(r + 8, w), pack_bf16x2(x[2], x[3]));
+      } else if ((tile % num_n) * BN < g.d2) {  // q / k
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int w = 4 * i + (lane & 3);
+          sts_u32(stage_tile + stage_off<512>(r, w), pack_bf16x2(acc[4 * i] * rs0, acc[4 * i + 1] * rs0));
+          sts_u32(stage_tile + stage_off<512>(r + 8, w), pack_bf16x2(acc[4 * i + 2] * rs1, acc[4 * i + 3] * rs1));
+        }
+      } else {
+        // v, transposed: tile column c is d-row c of v^T.  The lanes 4 apart hold tile rows r and r + 1 (r even) of
+        // the same two columns; they swap their packed pairs, and each stores one column's two rows as one word: the
+        // even row's lane column 8 i + 2 (l % 4), the odd row's lane the column after it.
+        const bool odd = (lane >> 2) & 1;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int c = 8 * i + 2 * (lane & 3) + (odd ? 1 : 0);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float rsr = h ? rs1 : rs0;
+            const uint32_t own = pack_bf16x2(acc[4 * i + 2 * h] * rsr, acc[4 * i + 2 * h + 1] * rsr);
+            const uint32_t peer = __shfl_xor_sync(0xffffffffu, own, 4);
+            sts_u32(stage_tile + stage_off<256>(c, (r + 8 * h) >> 1),
+                    odd ? __byte_perm(peer, own, 0x7632) : __byte_perm(own, peer, 0x5410));
+          }
+        }
       }
       mbar_arrive(out_full);
     }
@@ -721,11 +765,11 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
     // ===================== epilogue =====================
     const int e = warp - 8;
     __nv_bfloat16* const out = reinterpret_cast<__nv_bfloat16*>(g.out);
-    const int pitch = g.N / 2;
+    const int pitch = EPI == VNB_EPI_GEGLU ? g.N / 2 : g.d2;
     auto row_scales = [&](int tile) {  // row scales of `tile` into srs, then hand the staging tile to the consumers
       if (tile < tiles) {
         const int m0 = (tile / num_n) * BM;
-        for (int j = e * 32 + lane; j < BM; j += 32 * GG_EPI_WARPS) srs[j] = row_scale(g, m0 + j);
+        for (int j = e * 32 + lane; j < BM; j += 32 * PERS_EPI_WARPS) srs[j] = row_scale(g, m0 + j);
       }
       mbar_arrive(out_free);
     };
@@ -734,13 +778,61 @@ gemm_geglu_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gr
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
       const int m0 = (tile / num_n) * BM, n0 = (tile % num_n) * BN;
       mbar_wait(out_full, it & 1u);
-      // two tile rows per warp instruction: lane -> (row 2 u + lane / 16, 16-byte unit lane % 16)
+      if constexpr (EPI == VNB_EPI_GEGLU) {
+        // two tile rows per warp instruction: lane -> (row 2 u + lane / 16, 16-byte unit lane % 16)
 #pragma unroll 4
-      for (int u = e; u < BM / 2; u += GG_EPI_WARPS) {
-        const int rr = 2 * u + (lane >> 4);
-        const float4 v = lds_f4(stage_tile + gg_stage_off(rr, 4 * (lane & 15)));
-        if (m0 + rr < g.M)
-          *reinterpret_cast<float4*>(out + static_cast<size_t>(m0 + rr) * pitch + (n0 >> 1) + 8 * (lane & 15)) = v;
+        for (int u = e; u < BM / 2; u += PERS_EPI_WARPS) {
+          const int rr = 2 * u + (lane >> 4);
+          const float4 v = lds_f4(stage_tile + stage_off<256>(rr, 4 * (lane & 15)));
+          if (m0 + rr < g.M)
+            *reinterpret_cast<float4*>(out + static_cast<size_t>(m0 + rr) * pitch + (n0 >> 1) + 8 * (lane & 15)) = v;
+        }
+      } else if (n0 < g.d2) {
+        // q / k: one 512-byte tile row per warp instruction
+#pragma unroll 4
+        for (int rr = e; rr < BM; rr += PERS_EPI_WARPS) {
+          const float4 v = lds_f4(stage_tile + stage_off<512>(rr, 4 * lane));
+          if (m0 + rr < g.M)
+            *reinterpret_cast<float4*>(out + static_cast<size_t>(m0 + rr) * pitch + n0 + 8 * lane) = v;
+        }
+      } else {
+        // v^T: lane -> tile rows 4 lane .. 4 lane + 3 of every d-row, so a warp instruction stores a d-row's run of t.
+        // Their (b, t), bounds and frames select do not depend on the d-row.  Four rows of one batch row whose first
+        // t is a multiple of 4 go as one 8-byte store; any other group (a batch-row boundary, an odd T) element by
+        // element.  A frame past its call's own length is stored as 0 (a select, as in the one-tile epilogue).
+        const int d = g.N - g.d2;
+        uint16_t* const vt = reinterpret_cast<uint16_t*>(g.out2) + static_cast<size_t>(n0 - g.d2) * g.Tpad;
+        size_t off[4];
+        bool ok[4];
+        int bk[4];
+        uint32_t keep[2] = {0xffffffffu, 0xffffffffu};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int m = m0 + 4 * lane + k;
+          bk[k] = m / g.T;
+          const int t = m - bk[k] * g.T;
+          ok[k] = m < g.M;
+          off[k] = static_cast<size_t>(bk[k]) * d * g.Tpad + t;
+          if (ok[k] && g.frames != nullptr && t >= __ldg(g.frames + bk[k])) keep[k >> 1] &= (k & 1) ? 0xffffu : 0xffff0000u;
+        }
+        const bool wide = ok[3] && bk[3] == bk[0] && (off[0] & 3) == 0 && (g.Tpad & 3) == 0 &&
+                          (reinterpret_cast<uintptr_t>(g.out2) & 7) == 0;
+#pragma unroll 2
+        for (int c = e; c < BN; c += PERS_EPI_WARPS) {
+          uint2 v = lds_u2(stage_tile + stage_off<256>(c, 2 * lane));
+          v.x &= keep[0];
+          v.y &= keep[1];
+          uint16_t* const o = vt + static_cast<size_t>(c) * g.Tpad;
+          if (wide) {
+            *reinterpret_cast<uint2*>(o + off[0]) = v;
+          } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint32_t w = k < 2 ? v.x : v.y;
+              if (ok[k]) o[off[k]] = static_cast<uint16_t>((k & 1) ? (w >> 16) : w);
+            }
+          }
+        }
       }
       row_scales(tile + gridDim.x);
     }
@@ -780,8 +872,8 @@ static cudaError_t init_epi() {
     e = cudaFuncSetAttribute(gemm_wgmma_kernel<EPI, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM);
     if (e != cudaSuccess) return e;
   }
-  if constexpr (EPI == VNB_EPI_GEGLU) {
-    e = cudaFuncSetAttribute(gemm_geglu_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GG_SMEM);
+  if constexpr (EPI == VNB_EPI_GEGLU || EPI == VNB_EPI_QKV) {
+    e = cudaFuncSetAttribute(gemm_persistent_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, pers_smem<EPI>());
     if (e != cudaSuccess) return e;
   }
   if constexpr (EPI == VNB_EPI_SAMPLE) {
@@ -825,8 +917,8 @@ int get_gemm_max_clusters() {
 }
 
 // One CTA per output tile (the accumulator tile overlays the operand ring, so a CTA does not start a second tile), except
-// for the FFN-up GEMM without adapters: the persistent kernel, one CTA per SM (the SM count is cached by prepare_gemm(),
-// so none is queried inside a capture).
+// for the FFN-up and QKV GEMMs without adapters: the persistent kernel, one CTA per SM (the SM count is cached by
+// prepare_gemm(), so none is queried inside a capture).
 template <int EPI, bool ADAPT = false, bool SPLIT = false>
 static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t st) {
   cudaError_t e = init_epi<EPI>();
@@ -845,9 +937,9 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
     return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<EPI, true, ADAPT, SPLIT>, p.tmA, p.tmBh, g);
   }
   const int tiles = ((g.M + BM - 1) / BM) * (g.N / BN);
-  if constexpr (EPI == VNB_EPI_GEGLU && !ADAPT) {
+  if constexpr ((EPI == VNB_EPI_GEGLU || EPI == VNB_EPI_QKV) && !ADAPT) {
     const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-    gemm_geglu_persistent_kernel<<<grid, GG_THREADS, GG_SMEM, st>>>(p.tmA, p.tmB, g);
+    gemm_persistent_kernel<EPI><<<grid, PERS_THREADS, pers_smem<EPI>(), st>>>(p.tmA, p.tmB, g);
     return cudaGetLastError();
   }
   gemm_wgmma_kernel<EPI, false, ADAPT, SPLIT><<<tiles, GEMM_THREADS, GEMM_SMEM, st>>>(p.tmA, p.tmB, g);
