@@ -469,6 +469,26 @@ int32_t vnb_onset_detect(const float* samples, int32_t B, int32_t N, int32_t sr,
  * a NULL buffer. */
 int32_t vnb_onset_mask(const int32_t* onsets, const int32_t* counts, int32_t onset_rows, int32_t F, int32_t width,
                        int64_t* mask, int32_t B, int32_t C, int32_t T, void* stream);
+/* ---- beat tracking (librosa 0.10.1 beat.beat_track(y, sr, hop_length=hop) with start_bpm, tightness and trim as
+ *      given, frame units, restated on the device; DESIGN.md §10).  Nothing here synchronises. ----------------------
+ * samples (B, N) fp32 DEVICE, one clip per row; F = 1 + N / hop frames.  Each row is analysed on its own, so a row's
+ * results equal that row run alone, bit for bit.  Outputs (DEVICE): envelope (B, F) fp32 onset strength (the median
+ * over the 128 mel bands of the clamped dB flux); tempo (B) float64 BPM, 0 for an all-zero envelope; beats (B, F)
+ * int32, row b's first counts[b] entries are its beat frames in increasing order.  Everything after the envelope is
+ * float64.  workspace: DEVICE, at least vnb_beat_workspace_bytes(B, N, hop) bytes.  The float64 tables are built on
+ * the host on the first call for a (device, sr, hop) and cached; that first call allocates and uploads them.
+ * Refused: B outside 1..65535; N, sr or hop < 1; start_bpm or tightness <= 0; an 8 s tempo window int(8 sr) // hop
+ * outside 2..4096 frames; a NULL buffer; a workspace that is too small. */
+int32_t vnb_beat_workspace_bytes(int32_t B, int32_t N, int32_t hop, uint64_t* bytes);
+int32_t vnb_beat_track(const float* samples, int32_t B, int32_t N, int32_t sr, int32_t hop, double start_bpm,
+                       double tightness, int32_t trim, void* workspace, uint64_t workspace_bytes, float* envelope,
+                       double* tempo, int32_t* beats, int32_t* counts, void* stream);
+/* test hook: the tempo and beat decisions of vnb_beat_track from a caller's fp32 envelope (B, F) DEVICE.  workspace:
+ * vnb_beat_workspace_bytes(B, (F - 1) * hop + 1, hop) bytes.  The same refusals, with F < 1 in place of N < 1. */
+int32_t vnb_dbg_beat_from_envelope(const float* envelope, int32_t B, int32_t F, int32_t sr, int32_t hop,
+                                   double start_bpm, double tightness, int32_t trim, void* workspace,
+                                   uint64_t workspace_bytes, double* tempo, int32_t* beats, int32_t* counts,
+                                   void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

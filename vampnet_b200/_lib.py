@@ -144,6 +144,13 @@ _SIGS = {
                                      C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vnb_onset_mask": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                    C.c_int32, C.c_int32, C.c_void_p]),
+    "vnb_beat_workspace_bytes": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    "vnb_beat_track": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,
+                                   C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
+    "vnb_dbg_beat_from_envelope": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                               C.c_double, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
     "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,

@@ -94,6 +94,15 @@ class AudioSignal:
         self.audio_data = self.audio_data.mean(1, keepdim=True)
         return self
 
+    def trim(self, before: int, after: int):
+        """Drop `before` samples at the start and `after` at the end, in place (audiotools' trim: after == 0 keeps the
+        end, a negative count is a Python slice bound)."""
+        if after == 0:
+            self.audio_data = self.audio_data[..., before:]
+        else:
+            self.audio_data = self.audio_data[..., before:-after]
+        return self
+
     def resample(self, sample_rate: int):
         """Band-limited (Kaiser-windowed sinc) polyphase resampling as one strided conv."""
         sample_rate = int(sample_rate)

@@ -1243,4 +1243,55 @@ int32_t vnb_onset_mask(const int32_t* onsets, const int32_t* counts, int32_t ons
   return 0;
 }
 
+// ---- beat tracking (beat.cu) ----
+int32_t vnb_beat_workspace_bytes(int32_t B, int32_t N, int32_t hop, uint64_t* bytes) {
+  if (B < 1 || N < 1 || hop < 1 || !bytes) return fail("vnb_beat_workspace_bytes: need B >= 1, N >= 1, hop >= 1 and bytes");
+  *bytes = beat_workspace_bytes(B, 1 + N / hop);
+  return 0;
+}
+static int32_t beat_args(const char* fn, int32_t B, int32_t F, int32_t sr, int32_t hop, double start_bpm,
+                         double tightness, const void* in, const void* workspace, uint64_t workspace_bytes,
+                         const void* tempo, const void* beats, const void* counts, BeatTables* t) {
+  if (B < 1 || B > 65535) return fail("%s: need 1 <= B <= 65535 (got %d)", fn, B);
+  if (sr < 1 || hop < 1) return fail("%s: need sr >= 1 and hop >= 1 (got sr = %d, hop = %d)", fn, sr, hop);
+  if (!(start_bpm > 0) || !(tightness > 0)) return fail("%s: start_bpm and tightness must be > 0", fn);
+  if (!in || !workspace || !tempo || !beats || !counts) return fail("%s: a required buffer is NULL", fn);
+  const int W = beat_lags(sr, hop);
+  if (W < 2 || W > BEAT_MAX_LAGS)
+    return fail("%s: the 8 s tempo window is int(8 sr) // hop = %d frames; 2..%d are supported", fn, W, BEAT_MAX_LAGS);
+  const uint64_t need = beat_workspace_bytes(B, F);
+  if (workspace_bytes < need)
+    return fail("%s: workspace of %llu bytes, %llu needed", fn, (unsigned long long)workspace_bytes,
+                (unsigned long long)need);
+  CK(beat_tables(sr, hop, t));
+  return 0;
+}
+int32_t vnb_beat_track(const float* samples, int32_t B, int32_t N, int32_t sr, int32_t hop, double start_bpm,
+                       double tightness, int32_t trim, void* workspace, uint64_t workspace_bytes, float* envelope,
+                       double* tempo, int32_t* beats, int32_t* counts, void* stream) {
+  if (N < 1) return fail("vnb_beat_track: need N >= 1 (got %d)", N);
+  BeatTables bt;
+  if (int32_t rc = beat_args("vnb_beat_track", B, hop >= 1 ? 1 + N / hop : 1, sr, hop, start_bpm, tightness, samples,
+                             envelope ? workspace : nullptr, workspace_bytes, tempo, beats, counts, &bt))
+    return rc;
+  OnsetTables ot;
+  CK(onset_tables(sr, hop, &ot));
+  CK(launch_beat_track(samples, B, N, sr, hop, ot, bt, start_bpm, tightness, trim != 0, workspace, envelope, tempo,
+                       beats, counts, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_beat_from_envelope(const float* envelope, int32_t B, int32_t F, int32_t sr, int32_t hop,
+                                   double start_bpm, double tightness, int32_t trim, void* workspace,
+                                   uint64_t workspace_bytes, double* tempo, int32_t* beats, int32_t* counts,
+                                   void* stream) {
+  if (F < 1) return fail("vnb_dbg_beat_from_envelope: need F >= 1 (got %d)", F);
+  BeatTables bt;
+  if (int32_t rc = beat_args("vnb_dbg_beat_from_envelope", B, F, sr, hop, start_bpm, tightness, envelope, workspace,
+                             workspace_bytes, tempo, beats, counts, &bt))
+    return rc;
+  CK(launch_beat_from_envelope(envelope, B, F, sr, hop, bt, start_bpm, tightness, trim != 0, workspace, tempo, beats,
+                               counts, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 }  // extern "C"

@@ -204,5 +204,30 @@ cudaError_t launch_onset_detect(const float* samples, int B, int N, int hop, con
 // onset_rows == 1, else r = b; 1 elsewhere
 cudaError_t launch_onset_mask(const int32_t* onsets, const int32_t* counts, int onset_rows, int F, int width,
                               int64_t* mask, int B, int C, int T, cudaStream_t st);
+// samples (B, N) fp32 -> db (B, F, 128) mel dB: onset_spec_kernel alone (the first half of launch_onset_detect)
+cudaError_t launch_onset_spec(const float* samples, int B, int N, int hop, const OnsetTables& t, float* db,
+                              cudaStream_t st);
+
+// ---- beat tracking (beat.cu; librosa 0.10.1 beat_track restated, DESIGN.md §10) ----
+// the tempo estimate's autocorrelation window, W = int(8 sr) // hop lags, is supported for 2 <= W <= BEAT_MAX_LAGS
+constexpr int BEAT_MAX_LAGS = 4096;
+int beat_lags(int sr, int hop);
+// device tables (float64, built on the host once per (device, sr, hop), then cached)
+struct BeatTables {
+  const double* window;    // (W) periodic Hann
+  const double* bpm;       // (W) tempo_frequencies: inf, 60 sr / (hop k)
+  const double* log2_bpm;  // (W)
+  int W, max_idx;          // max_idx: the first lag below 320 BPM
+};
+cudaError_t beat_tables(int sr, int hop, BeatTables* out);
+size_t beat_workspace_bytes(int B, int F);
+// samples (B, N) fp32 -> env (B, F) fp32 onset strength (median over bands), tempo (B) BPM, beats (B, F) + counts (B)
+cudaError_t launch_beat_track(const float* samples, int B, int N, int sr, int hop, const OnsetTables& ot,
+                              const BeatTables& bt, double start_bpm, double tightness, int trim, void* workspace,
+                              float* env, double* tempo, int32_t* beats, int32_t* counts, cudaStream_t st);
+// the same decisions from a given envelope (B, F)
+cudaError_t launch_beat_from_envelope(const float* env, int B, int F, int sr, int hop, const BeatTables& bt,
+                                      double start_bpm, double tightness, int trim, void* workspace, double* tempo,
+                                      int32_t* beats, int32_t* counts, cudaStream_t st);
 
 }  // namespace vnb

@@ -305,6 +305,14 @@ cudaError_t launch_onset_detect(const float* samples, int B, int N, int hop, con
   return cudaGetLastError();
 }
 
+cudaError_t launch_onset_spec(const float* samples, int B, int N, int hop, const OnsetTables& t, float* db,
+                              cudaStream_t st) {
+  const int F = 1 + N / hop;
+  onset_spec_kernel<<<dim3(F, B), THREADS, 0, st>>>(samples, N, F, hop, t, db);
+  count_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t launch_onset_mask(const int32_t* onsets, const int32_t* counts, int onset_rows, int F, int width,
                               int64_t* mask, int B, int C, int T, cudaStream_t st) {
   const size_t n = (size_t)B * C * T;

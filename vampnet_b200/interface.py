@@ -17,6 +17,7 @@ import torch
 
 from . import mask as pmask
 from .audio import AudioSignal
+from .beats import BeatTracker, beat_mask
 from .mask import *  # noqa: F401,F403  (reference does `from .mask import *`, interface.py:13)
 from .modules.transformer import VampNet
 
@@ -73,10 +74,11 @@ class Interface(torch.nn.Module):
         else:
             self.c2f_path = None
             self.c2f = None
-        # WaveBeat (interface.py:96-101) is a separate model outside the hot path (SURVEY.md §2 row 9)
-        self.beat_tracker = None
+        # WaveBeat (interface.py:96-101) is a separate network whose package is not available; beat masks use the
+        # librosa-style tracker of beats.py instead (any object with extract_beats can be assigned in its place)
+        self.beat_tracker = BeatTracker(device)
         if wavebeat_ckpt is not None and Path(wavebeat_ckpt).exists():
-            logging.debug("wavebeat checkpoint present but the beat tracker is out of scope; beat masks disabled")
+            logging.debug("wavebeat checkpoint ignored: beat masks use the built-in librosa-style beat tracker")
         self.device = device
         self.loudness = -24.0
         # `compile` (torch.compile in the reference, interface.py:107-112) is accepted and ignored:
@@ -92,7 +94,7 @@ class Interface(torch.nn.Module):
         if c2f is not None:
             self.c2f.chunk_size_s = coarse2fine_chunk_size_s
         self.codec_path = self.coarse_path = self.c2f_path = None
-        self.beat_tracker = None
+        self.beat_tracker = BeatTracker(device)
         self.device = device
         self.loudness = -24.0
         return self.to(device)
@@ -177,6 +179,8 @@ class Interface(torch.nn.Module):
         self.codec.to(device)
         if self.c2f is not None:
             self.c2f.to(device)
+        if isinstance(self.beat_tracker, BeatTracker):
+            self.beat_tracker.device = device
         return self
 
     def set_chunk_size(self, chunk_size_s: float):
@@ -214,9 +218,33 @@ class Interface(torch.nn.Module):
         enc = self.codec.encode_many([s.samples for s in prepared], [s.sample_rate for s in prepared])
         return [e["codes"] for e in enc]
 
-    def make_beat_mask(self, *a, **k):
-        raise RuntimeError("make_beat_mask needs the WaveBeat tracker (interface.py:226-322), a separate model "
-                           "outside the hot path (SURVEY.md §2 row 9)")
+    # ------------------------------------------------------------------ beats (interface.py:226-322)
+    def snap_to_beats(self, signal: AudioSignal):
+        """The signal trimmed to start at the first beat and end at the last."""
+        assert hasattr(self, "beat_tracker"), "No beat tracker loaded"
+        beats, downbeats = self.beat_tracker.extract_beats(signal)
+        samples_begin = int(beats[0] * signal.sample_rate)
+        samples_end = int(beats[-1] * signal.sample_rate)
+        return signal.clone().trim(samples_begin, signal.length - samples_end)
+
+    def make_beat_mask(self, signal: AudioSignal = None, before_beat_s: float = 0.0, after_beat_s: float = 0.02,
+                       mask_downbeats: bool = True, mask_upbeats: bool = True, downbeat_downsample_factor: int = None,
+                       beat_downsample_factor: int = None, dropout: float = 0.0, invert: bool = True):
+        """A mask that keeps (0 after the inversion) the codes at and around each beat: before_beat_s before it,
+        after_beat_s after it.  The beat times come from self.beat_tracker (librosa-style by default: no downbeats,
+        so beat_downsample_factor thins all beats); the mask is built from them as the reference builds it."""
+        if torch.device(self.device).type != "cuda":
+            raise RuntimeError(f"make_beat_mask: the beat tracker runs on a CUDA device; this Interface is on "
+                               f"{self.device}")
+        assert self.beat_tracker is not None, "No beat tracker loaded"
+        if signal is None:
+            raise TypeError("make_beat_mask: a signal is required")
+        beats, downbeats = self.beat_tracker.extract_beats(signal)
+        n_codebooks = self.c2f.n_codebooks if self.c2f is not None else self.coarse.n_codebooks
+        return beat_mask(beats, downbeats, signal.duration, self.s2t, n_codebooks, self.device,
+                         before_beat_s=before_beat_s, after_beat_s=after_beat_s, mask_downbeats=mask_downbeats,
+                         mask_upbeats=mask_upbeats, downbeat_downsample_factor=downbeat_downsample_factor,
+                         beat_downsample_factor=beat_downsample_factor, dropout=dropout, invert=invert)
 
     # ------------------------------------------------------------------ chunk helpers
     @staticmethod
