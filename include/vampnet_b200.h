@@ -489,6 +489,24 @@ int32_t vnb_dbg_beat_from_envelope(const float* envelope, int32_t B, int32_t F, 
                                    double start_bpm, double tightness, int32_t trim, void* workspace,
                                    uint64_t workspace_bytes, double* tempo, int32_t* beats, int32_t* counts,
                                    void* stream);
+/* ---- pitch shift (torch_pitch_shift 1.2's pitch_shift: torch.stft -> torchaudio.functional.phase_vocoder ->
+ *      torch.istft -> torchaudio.functional.resample, restated on the device; DESIGN.md §11).  Nothing here
+ *      synchronises. -------------------------------------------------------------------------------------------------
+ * samples and out (rows, N) fp32 DEVICE, each row shifted on its own with fixed-order reductions, so a row's result
+ * equals that row run alone, bit for bit.  The caller passes what the Python wrapper derives from the shift:
+ * new_freq = int(sample_rate / ratio) and rate = float(1 / ratio); the library derives the frame counts, the istft
+ * length and the gcd of the two rates.  Everything between the fp32 ends is float64.  workspace: DEVICE, at least
+ * vnb_pitch_workspace_bytes(...) bytes (about 0.6 GB per 10 s row at 44.1 kHz and +12 semitones).  The float64 DFT
+ * bases are built on the host on the first call for a (device, n_fft) and cached; that first call allocates and
+ * uploads them.  Refused: a NULL buffer, a workspace that is too small, rows outside 1..65535, n_fft outside 16..4096,
+ * hop < 1 or hop > n_fft, N <= n_fft / 2, sample_rate or new_freq < 1, rate <= 0 or not finite. */
+int32_t vnb_pitch_workspace_bytes(int32_t rows, int32_t N, int32_t sample_rate, int32_t new_freq, int32_t n_fft,
+                                  int32_t hop, double rate, uint64_t* bytes);
+int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t sample_rate, int32_t new_freq,
+                        int32_t n_fft, int32_t hop, double rate, void* workspace, uint64_t workspace_bytes, float* out,
+                        void* stream);
+/* test hook: the phase vocoder's time steps, out[i] = float(rate) * float(i) for i < n, fp32 DEVICE */
+int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

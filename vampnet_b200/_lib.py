@@ -151,6 +151,10 @@ _SIGS = {
     "vnb_dbg_beat_from_envelope": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
                                                C.c_double, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p]),
+    "vnb_pitch_workspace_bytes": (C.c_int32, [C.c_int32] * 6 + [C.c_double, C.POINTER(C.c_uint64)]),
+    "vnb_pitch_shift": (C.c_int32, [C.c_void_p] + [C.c_int32] * 6 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                                      C.c_void_p]),
+    "vnb_dbg_pitch_time_steps": (C.c_int32, [C.c_double, C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
     "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,

@@ -3,6 +3,7 @@
 #include <cuda_bf16.h>
 #include <cudaTypedefs.h>
 
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -1291,6 +1292,48 @@ int32_t vnb_dbg_beat_from_envelope(const float* envelope, int32_t B, int32_t F, 
     return rc;
   CK(launch_beat_from_envelope(envelope, B, F, sr, hop, bt, start_bpm, tightness, trim != 0, workspace, tempo, beats,
                                counts, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+// ---- pitch shift (pitch.cu) ----
+static int32_t pitch_args(const char* fn, int32_t rows, int32_t N, int32_t sr, int32_t new_freq, int32_t n_fft,
+                          int32_t hop, double rate, PitchPlan* p) {
+  if (rows < 1 || rows > 65535) return fail("%s: need 1 <= rows <= 65535 (got %d)", fn, rows);
+  if (n_fft < PITCH_MIN_NFFT || n_fft > PITCH_MAX_NFFT)
+    return fail("%s: n_fft = %d; %d..%d are supported", fn, n_fft, PITCH_MIN_NFFT, PITCH_MAX_NFFT);
+  if (hop < 1 || hop > n_fft) return fail("%s: need 1 <= hop <= n_fft (got hop = %d, n_fft = %d)", fn, hop, n_fft);
+  if (N <= n_fft / 2) return fail("%s: need N > n_fft // 2 for the reflect padding (got N = %d, n_fft = %d)", fn, N, n_fft);
+  if (sr < 1 || new_freq < 1) return fail("%s: need sample_rate >= 1 and new_freq >= 1 (got %d, %d)", fn, sr, new_freq);
+  if (!(rate > 0) || !std::isfinite(rate)) return fail("%s: need a finite rate > 0 (got %g)", fn, rate);
+  if (pitch_plan(rows, N, sr, new_freq, n_fft, hop, rate, p))
+    return fail("%s: ceil(F / rate) stretched frames is out of range (N = %d, hop = %d, rate = %g)", fn, N, hop, rate);
+  return 0;
+}
+int32_t vnb_pitch_workspace_bytes(int32_t rows, int32_t N, int32_t sr, int32_t new_freq, int32_t n_fft, int32_t hop,
+                                  double rate, uint64_t* bytes) {
+  if (!bytes) return fail("vnb_pitch_workspace_bytes: bytes is NULL");
+  PitchPlan p;
+  if (int32_t rc = pitch_args("vnb_pitch_workspace_bytes", rows, N, sr, new_freq, n_fft, hop, rate, &p)) return rc;
+  *bytes = pitch_workspace_bytes(p);
+  return 0;
+}
+int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t sr, int32_t new_freq, int32_t n_fft,
+                        int32_t hop, double rate, void* workspace, uint64_t workspace_bytes, float* out, void* stream) {
+  if (!samples || !workspace || !out) return fail("vnb_pitch_shift: samples, workspace and out are required");
+  PitchPlan p;
+  if (int32_t rc = pitch_args("vnb_pitch_shift", rows, N, sr, new_freq, n_fft, hop, rate, &p)) return rc;
+  const uint64_t need = pitch_workspace_bytes(p);
+  if (workspace_bytes < need)
+    return fail("vnb_pitch_shift: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
+                (unsigned long long)need);
+  const double *fwd = nullptr, *inv = nullptr;
+  CK(pitch_basis(n_fft, &fwd, &inv));
+  CK(launch_pitch_shift(samples, p, fwd, inv, workspace, out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* stream) {
+  if (!out || n < 1 || !(rate > 0)) return fail("vnb_dbg_pitch_time_steps: need out, n >= 1 and rate > 0");
+  CK(launch_pitch_time_steps((float)rate, n, out, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 

@@ -230,4 +230,26 @@ cudaError_t launch_beat_from_envelope(const float* env, int B, int F, int sr, in
                                       double start_bpm, double tightness, int trim, void* workspace, double* tempo,
                                       int32_t* beats, int32_t* counts, cudaStream_t st);
 
+// ---- pitch shift (pitch.cu; torch_pitch_shift's stft -> phase vocoder -> istft -> resample restated, DESIGN.md §11) ----
+constexpr int PITCH_MIN_NFFT = 16, PITCH_MAX_NFFT = 4096;
+// shapes of one call: F = 1 + (N + 2 (n_fft / 2) - n_fft) / hop STFT frames, F2 = ceil(F / rate) stretched frames (F when rate == 1), L the
+// istft length, target the resampled length before the cut or pad to N
+struct PitchPlan {
+  int rows = 0, N = 0, sr = 0, new_freq = 0, n_fft = 0, hop = 0, nb = 0, F = 0, F2 = 0, nchunks = 0, width = 0;
+  double rate = 1.0, base = 0.0, scale = 0.0;
+  long long L = 0, target = 0, orig_g = 1, new_g = 1;
+  bool stretch = false, resample = false;
+};
+// 0, or 1 when the stretched frame count is out of range
+int pitch_plan(int rows, int N, int sr, int new_freq, int n_fft, int hop, double rate, PitchPlan* p);
+size_t pitch_workspace_bytes(const PitchPlan& p);
+// float64 forward (n_fft x 2 n_bins) and inverse (2 n_bins x n_fft) DFT bases, zero padded to the GEMM tiles; built on
+// the host once per (device, n_fft), then cached
+cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv);
+// samples (rows, N) fp32 -> out (rows, N) fp32
+cudaError_t launch_pitch_shift(const float* x, const PitchPlan& p, const double* fwd, const double* inv, void* ws,
+                               float* out, cudaStream_t st);
+// the vocoder's time steps: out[i] = float(rate) * float(i), i < n
+cudaError_t launch_pitch_time_steps(float rate, long long n, float* out, cudaStream_t st);
+
 }  // namespace vnb
