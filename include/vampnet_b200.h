@@ -507,6 +507,38 @@ int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t s
                         void* stream);
 /* test hook: the phase vocoder's time steps, out[i] = float(rate) * float(i) for i < n, fp32 DEVICE */
 int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* stream);
+/* ---- validation metrics (the reference's scripts/exp/train.py val_loop / _metrics / accuracy, train.py:155-213,
+ *      327-371; DESIGN.md §12).  Nothing here synchronises. -----------------------------------------------------------
+ * logits (B, S, V) fp32 DEVICE, 16-byte aligned, as vnb_forward_codes writes them, S = T * (C - ncc), row s = t * (C -
+ * ncc) + c.  z and mask (B, C, T) int64 DEVICE: row (b, s)'s target is z[b, ncc + s % (C - ncc), s / (C - ncc)], it is
+ * masked where mask at the same place is not 0.  r (B) float64 DEVICE, each item's mask ratio.  Writes out9, fp32
+ * DEVICE, in the reference's key order:
+ *   [0] loss: CrossEntropyLoss(label_smoothing, ignore_index) over the masked rows, ((1 - ls) sum nll + ls sum smooth) /
+ *       n with nll = lse - x[target] and smooth = lse - mean(x), summed in float64 and rounded to fp32 once; NaN when
+ *       no row is masked;
+ *   [1 + 4 range + 2 k + sel] accuracy over the rows of the items whose r lies in range 0 = [0, 0.5) or 1 = [0.5, 1.0)
+ *       (r = 1.0 is in neither), k 0 = top-1 or 1 = top-25, sel 0 = unmasked or 1 = masked rows: the share of rows
+ *       whose target is in the top k, NaN for an empty selection.  A row with gt = #{x > x[target]} and eq = #{other
+ *       x == x[target]} is correct iff gt + eq < k; a row with gt < k <= gt + eq (a tie at the k-th place, which
+ *       torch.topk breaks in an implementation-defined way) counts as not correct and, when ambiguous is not NULL, in
+ *       ambiguous[i], int32 DEVICE (9; ambiguous[0] = 0).
+ * A code outside 0..V-1 cannot be refused without a host read: it makes the loss NaN, and every accuracy whose
+ * selection holds its row.  Every reduction has a fixed order: two calls give the same bits, and a row's record
+ * (vnb_dbg_xent_rows) equals that row run in a batch of one.  workspace: DEVICE, at least
+ * vnb_xent_metrics_workspace_bytes(B, S) bytes.  Refused: a NULL buffer, B, C or T < 1, ncc outside 0..C-1, V outside
+ * 1..1024 or not a multiple of 4, label_smoothing outside [0, 1] or NaN, a workspace that is too small, logits not
+ * 16-byte aligned. */
+typedef struct vnb_xent_row {
+  double nll, smooth; /* NaN for an out-of-range code */
+  int32_t gt, eq;     /* -1 for an out-of-range code */
+} vnb_xent_row;
+int32_t vnb_xent_metrics_workspace_bytes(int32_t B, int64_t S, uint64_t* bytes);
+int32_t vnb_xent_metrics(const float* logits, const int64_t* z, const int64_t* mask, const double* r, int32_t B,
+                         int32_t C, int32_t T, int32_t ncc, int32_t V, double label_smoothing, void* workspace,
+                         uint64_t workspace_bytes, float* out9, int32_t* ambiguous, void* stream);
+/* test hook: the per-row records (B * S vnb_xent_row, DEVICE) of vnb_xent_metrics; same refusals */
+int32_t vnb_dbg_xent_rows(const float* logits, const int64_t* z, int32_t B, int32_t C, int32_t T, int32_t ncc,
+                          int32_t V, vnb_xent_row* rows, void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

@@ -155,6 +155,10 @@ _SIGS = {
     "vnb_pitch_shift": (C.c_int32, [C.c_void_p] + [C.c_int32] * 6 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,
                                                                       C.c_void_p]),
     "vnb_dbg_pitch_time_steps": (C.c_int32, [C.c_double, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_xent_metrics_workspace_bytes": (C.c_int32, [C.c_int32, C.c_int64, C.POINTER(C.c_uint64)]),
+    "vnb_xent_metrics": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32] * 5 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                                          C.c_void_p, C.c_void_p]),
+    "vnb_dbg_xent_rows": (C.c_int32, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
     "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,

@@ -1337,4 +1337,43 @@ int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* strea
   return 0;
 }
 
+// ---- validation metrics (validate.cu) ----
+static int32_t xent_args(const char* fn, const float* logits, int32_t B, int32_t C, int32_t T, int32_t ncc, int32_t V) {
+  if (B < 1 || C < 1 || T < 1) return fail("%s: need B, C, T >= 1 (got %d, %d, %d)", fn, B, C, T);
+  if (ncc < 0 || ncc >= C) return fail("%s: need 0 <= ncc < C (got ncc = %d, C = %d)", fn, ncc, C);
+  if (V < 1 || V > XENT_MAX_V || V % 4)
+    return fail("%s: V = %d; a multiple of 4 in 1..%d is supported", fn, V, XENT_MAX_V);
+  if (reinterpret_cast<uintptr_t>(logits) % 16) return fail("%s: logits must be 16-byte aligned", fn);
+  return 0;
+}
+int32_t vnb_xent_metrics_workspace_bytes(int32_t B, int64_t S, uint64_t* bytes) {
+  if (!bytes) return fail("vnb_xent_metrics_workspace_bytes: bytes is NULL");
+  if (B < 1 || S < 1) return fail("vnb_xent_metrics_workspace_bytes: need B, S >= 1 (got %d, %lld)", B, (long long)S);
+  *bytes = xent_workspace_bytes(B, S);
+  return 0;
+}
+int32_t vnb_xent_metrics(const float* logits, const int64_t* z, const int64_t* mask, const double* r, int32_t B,
+                         int32_t C, int32_t T, int32_t ncc, int32_t V, double label_smoothing, void* workspace,
+                         uint64_t workspace_bytes, float* out9, int32_t* ambiguous, void* stream) {
+  if (!logits || !z || !mask || !r || !workspace || !out9)
+    return fail("vnb_xent_metrics: logits, z, mask, r, workspace and out9 are required");
+  if (int32_t rc = xent_args("vnb_xent_metrics", logits, B, C, T, ncc, V)) return rc;
+  if (!(label_smoothing >= 0.0 && label_smoothing <= 1.0))
+    return fail("vnb_xent_metrics: need 0 <= label_smoothing <= 1 (got %g)", label_smoothing);
+  const uint64_t need = xent_workspace_bytes(B, (long long)T * (C - ncc));
+  if (workspace_bytes < need)
+    return fail("vnb_xent_metrics: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
+                (unsigned long long)need);
+  CK(launch_xent_metrics(logits, z, mask, r, B, C, T, ncc, V, label_smoothing, workspace, out9, ambiguous,
+                         reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_xent_rows(const float* logits, const int64_t* z, int32_t B, int32_t C, int32_t T, int32_t ncc,
+                          int32_t V, vnb_xent_row* rows, void* stream) {
+  if (!logits || !z || !rows) return fail("vnb_dbg_xent_rows: logits, z and rows are required");
+  if (int32_t rc = xent_args("vnb_dbg_xent_rows", logits, B, C, T, ncc, V)) return rc;
+  CK(launch_xent_rows(logits, z, B, C, T, ncc, V, rows, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 }  // extern "C"

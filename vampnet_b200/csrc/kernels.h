@@ -252,4 +252,16 @@ cudaError_t launch_pitch_shift(const float* x, const PitchPlan& p, const double*
 // the vocoder's time steps: out[i] = float(rate) * float(i), i < n
 cudaError_t launch_pitch_time_steps(float rate, long long n, float* out, cudaStream_t st);
 
+// ---- validation metrics (validate.cu; train.py's val_loop loss and _metrics accuracies, DESIGN.md §12) ----
+constexpr int XENT_MAX_V = 1024;
+using XentRow = vnb_xent_row;
+size_t xent_workspace_bytes(long long B, long long S);
+// logits (B, S, V) fp32 -> rows (B * S) records
+cudaError_t launch_xent_rows(const float* logits, const int64_t* z, int B, int C, int T, int ncc, int V, XentRow* rows,
+                             cudaStream_t st);
+// the records, then out (9) fp32 and, when not NULL, ambiguous (9) int32
+cudaError_t launch_xent_metrics(const float* logits, const int64_t* z, const int64_t* mask, const double* r, int B,
+                                int C, int T, int ncc, int V, double eps, void* workspace, float* out,
+                                int32_t* ambiguous, cudaStream_t st);
+
 }  // namespace vnb

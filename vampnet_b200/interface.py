@@ -218,6 +218,19 @@ class Interface(torch.nn.Module):
         enc = self.codec.encode_many([s.samples for s in prepared], [s.sample_rate for s in prepared])
         return [e["codes"] for e in enc]
 
+    # ------------------------------------------------------------------ validation (scripts/exp/train.py:327-371)
+    def validate(self, signal: AudioSignal, model: str = "coarse", **kwargs) -> dict:
+        """The reference training script's validation metrics for `signal`: encode(signal), then the coarse or c2f
+        model's VampNet.validate(codec, codes, **kwargs) (r / rng, mask, label_smoothing, adapter).  Returns the
+        reference's dict of 9 0-d fp32 device tensors ("loss", "accuracy-..."); held-out clips score a checkpoint or a
+        fine-tune registered with add_finetuned (adapter=name)."""
+        if model not in ("coarse", "c2f"):
+            raise ValueError(f"validate: model must be 'coarse' or 'c2f', got {model!r}")
+        vn = self.coarse if model == "coarse" else self.c2f
+        if vn is None:
+            raise ValueError("validate: this Interface has no c2f model")
+        return vn.validate(self.codec, self.encode(signal), **kwargs)
+
     # ------------------------------------------------------------------ beats (interface.py:226-322)
     def snap_to_beats(self, signal: AudioSignal):
         """The signal trimmed to start at the first beat and end at the last."""

@@ -619,6 +619,55 @@ class VampNet(nn.Module):
                                                                 _lib.ptr(logits), _lib.stream_ptr(self.device)))
         return logits
 
+    @torch.no_grad()
+    def validate(self, codec, z: torch.Tensor, r=None, mask: torch.Tensor = None, rng=None, label_smoothing: float = 0.1,
+                 adapter: str = None) -> dict:
+        """One validation step of the reference's training script (scripts/exp/train.py val_loop, :327-371) from codes.
+
+        z: (B, C', T) codes with C' >= n_codebooks; the first n_codebooks are used (train.py:334).  Pass exactly one of
+        r, each item's mask ratio (a number or a (B,) tensor), and rng, a torch.quasirandom.SobolEngine that draws it
+        as rng.draw(B)[:, 0] (train.py:339).  Without a mask the mask is pmask.random(z, r) with the conditioning
+        codebooks unmasked (the reference's torch calls, so the same RNG state gives the same mask); a given (B,
+        n_codebooks or C', T) binary mask is used as given.  The logits are forward_codes(apply_mask(z, mask)), with
+        adapter applied.
+
+        Returns the reference's dict: "loss", CrossEntropyLoss(label_smoothing, ignore_index=-100) over the masked
+        tokens, and "accuracy-{0-0.5,0.5-1.0}/top{1,25}/{unmasked,masked}", each a 0-d fp32 tensor on the model's
+        device.  Nothing from the forward to the returned dict synchronises."""
+        from .. import mask as pmask
+        from ..metrics import KEYS, xent_metrics
+        if z.ndim != 3 or z.shape[1] < self.n_codebooks:
+            raise ValueError(f"validate: z must be (B, C >= {self.n_codebooks}, T), got {tuple(z.shape)}")
+        if (r is None) == (rng is None):
+            raise ValueError("validate: pass exactly one of r and rng")
+        ls = float(label_smoothing)
+        if not 0.0 <= ls <= 1.0:
+            raise ValueError(f"validate: label_smoothing must be in [0, 1], got {label_smoothing}")
+        full_shape = tuple(z.shape)
+        B, T = z.shape[0], z.shape[-1]
+        dev = self.device
+        z = z[:, :self.n_codebooks].to(dev, torch.int64)
+        if rng is not None:
+            r = rng.draw(B)[:, 0]
+        elif not torch.is_tensor(r):
+            r = pmask._scalar_to_batch(r, B)
+        if tuple(r.shape) != (B,):
+            raise ValueError(f"validate: r must be a number or a ({B},) tensor, got shape {tuple(r.shape)}")
+        r = r.to(dev)
+        if mask is None:
+            mask = pmask.codebook_unmask(pmask.random(z, r), self.n_conditioning_codebooks)
+        else:
+            if tuple(mask.shape) not in (full_shape, (B, self.n_codebooks, T)):
+                raise ValueError(f"validate: mask {tuple(mask.shape)} must be (B, n_codebooks, T) = "
+                                 f"{(B, self.n_codebooks, T)} or z's shape {full_shape}")
+            mask = mask[:, :self.n_codebooks].to(dev, torch.int64)
+            if not bool(((mask == 0) | (mask == 1)).all()):
+                raise ValueError("validate: mask must be binary")
+        z_mask, mask = pmask.apply_mask(z, mask, self.mask_token, check=False)
+        logits = self.forward_codes(z_mask, codec, adapter=adapter)
+        out = xent_metrics(logits, z, mask, r, self.n_conditioning_codebooks, ls)
+        return {k: out[i] for i, k in enumerate(KEYS)}
+
     def hidden_state(self, B: int, T: int) -> torch.Tensor:
         """fp32 residual stream (B, T, d) after the last layer of the most recent forward of that shape (debug tap)."""
         out = torch.empty(B, T, self.embedding_dim, device=self.device, dtype=torch.float32)
