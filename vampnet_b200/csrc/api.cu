@@ -93,23 +93,24 @@ bool make_tmap_3d(CUtensorMap* tm, const void* base, uint64_t batch, uint64_t ro
   return true;
 }
 
-bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out, void* out2,
-                    const float* bias, int T, int Tpad, int d2) {
+// Fills a plan's tensor maps (A (M,K) bf16, W (N,K) bf16) and arguments, with the fused RMSNorm (DESIGN.md §4) wired as
+// in the forward: ss_in (non-null) makes the plan a consumer that scales its rows by rsqrt(mean(A^2) + eps) from ss_parts
+// partial row sums of squares; out_bf16 (non-null) a producer that also stores bf16(out) and its row sums of squares
+// to ss_out, the next GEMM's operand.
+static bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out,
+                           void* out2, const float* bias, int T, int Tpad, const float* ss_in, int ss_parts,
+                           float inv_d, float eps, void* out_bf16, float* ss_out) {
   if (N % 256 != 0 || K % 64 != 0 || M < 1) {
     g_tmap_err = "gemm: need N % 256 == 0 and K % 64 == 0";
     return false;
   }
-  p->M = M; p->N = N; p->K = K; p->epi = epi; p->out = out; p->out2 = out2; p->bias = bias;
-  p->T = T; p->Tpad = Tpad; p->d2 = d2;
+  GemmArgs& a = p->args;
+  a.M = M; a.N = N; a.K = K; a.epi = epi; a.out = out; a.out2 = out2; a.bias = bias;
+  a.T = T; a.Tpad = Tpad; a.d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;  // QKV: N = 3 d_model, v starts at 2 d_model
+  if (ss_in != nullptr) { a.ss_in = ss_in; a.ss_parts = ss_parts; a.inv_d = inv_d; a.eps = eps; }
+  a.out_bf16 = reinterpret_cast<__nv_bfloat16*>(out_bf16); a.ss_out = ss_out;
   return make_tmap_2d(&p->tmA, A, M, K, 128, 64) && make_tmap_2d(&p->tmB, W, N, K, 256, 64) &&
          make_tmap_2d(&p->tmBh, W, N, K, 128, 64);
-}
-
-// RESID plans that also produce the next GEMM's operand: bf16 copy of the updated rows + row sums of squares.
-bool gemm_plan_set_fused_out(GemmPlan* p, void* out_bf16, float* ss_out) {
-  p->out_bf16 = out_bf16;
-  p->ss_out = ss_out;
-  return true;
 }
 
 bool make_attn_plan(AttnPlan* p, const void* qk, const void* vT, void* out, const float* rel, int sat, int B, int T,
@@ -134,19 +135,21 @@ struct DevBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-struct GraphKey {  // graphs bake pointers, so generate() stages z/mask/out in workspace-owned buffers
-  int steps;
-  bool has_mask;
-  bool top_p;  // selects the sampler kernel variant
-  int variant;  // GEMM kernel variant baked into the graph (vnb_set_option "gemm_pair")
-  bool fused;   // sampler fused into the classifier epilogue (vnb_set_option "fused_sampler")
-  bool adapted;  // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
-  bool ragged;   // QKV and attention read the frames table (some group is shorter than T)
-  bool mixed_steps;  // every kernel of iteration i reads the live table (some group has fewer steps than the launch)
-  bool split;        // nucleus and plain groups in one fused launch: split classifier epilogue and sampler
-  bool operator<(const GraphKey& o) const {
-    return std::tie(steps, has_mask, top_p, variant, fused, adapted, ragged, mixed_steps, split) <
-           std::tie(o.steps, o.has_mask, o.top_p, o.variant, o.fused, o.adapted, o.ragged, o.mixed_steps, o.split);
+// Which kernels a launch runs.  It is also the key of a captured generate graph (graphs bake pointers, so generate()
+// stages z/mask/out in workspace-owned buffers); a forward runs the default.
+struct Variant {
+  int steps = 0;          // generate iterations
+  bool has_mask = false;
+  bool top_p = false;     // selects the sampler kernel variant
+  int gemm_pair = 0;      // GEMM kernel variant baked into the graph (vnb_set_option "gemm_pair")
+  bool fused = false;     // sampler fused into the classifier epilogue (vnb_set_option "fused_sampler")
+  bool adapted = false;   // LoRA down-projections + adapted GEMM epilogues (some group has an adapter)
+  bool ragged = false;    // QKV and attention read the frames table (some group is shorter than T)
+  bool mixed_steps = false;  // every kernel of iteration i reads the live table (some group has fewer steps than S)
+  bool split = false;        // nucleus and plain groups in one fused launch: split classifier epilogue and sampler
+  bool operator<(const Variant& o) const {
+    return std::tie(steps, has_mask, top_p, gemm_pair, fused, adapted, ragged, mixed_steps, split) <
+           std::tie(o.steps, o.has_mask, o.top_p, o.gemm_pair, o.fused, o.adapted, o.ragged, o.mixed_steps, o.split);
   }
 };
 
@@ -173,8 +176,8 @@ struct Workspace {
   GemmPlan cls_sample;  // the classifier with the sampling epilogue (generate loop)
   bool can_fuse = false;
   AttnPlan attn;
-  std::map<GraphKey, cudaGraphExec_t> graphs;
-  std::map<GraphKey, unsigned long long> graph_kernels;
+  std::map<Variant, cudaGraphExec_t> graphs;
+  std::map<Variant, unsigned long long> graph_kernels;
   ~Workspace() { for (auto& kv : graphs) cudaGraphExecDestroy(kv.second); }
 };
 
@@ -276,45 +279,44 @@ static int get_workspace(vnb_model* m, int B, int T, Workspace** out) {
   ws->qkv.resize(L); ws->wo.resize(L); ws->up.resize(L); ws->down.resize(L);
   const size_t dd = static_cast<size_t>(d) * d;
   const float inv_d = 1.0f / static_cast<float>(d), eps = 1e-6f;
-  auto consumer = [&](GemmPlan& p, const DevBuf& ss) { p.ss_in = ss.as<float>(); p.ss_parts = ws->ss_parts; p.inv_d = inv_d; p.eps = eps; };
-  auto producer = [&](GemmPlan& p, const DevBuf& ss) { return gemm_plan_set_fused_out(&p, ws->y.p, ss.as<float>()); };
+  // ss_in: the row sums of squares a consumer's A operand came with; ss_out: where a producer leaves them, with bf16(x) in y
+  auto plan = [&](GemmPlan& p, int epi, const void* A, const void* W, int N, int K, void* out, void* out2,
+                  const float* bias, const DevBuf* ss_in, const DevBuf* ss_out) {
+    return make_gemm_plan(&p, epi, A, W, ws->M, N, K, out, out2, bias, T, ws->Tpad,
+                          ss_in ? ss_in->as<float>() : nullptr, ws->ss_parts, inv_d, eps, ss_out ? ws->y.p : nullptr,
+                          ss_out ? ss_out->as<float>() : nullptr);
+  };
   for (int l = 0; l < L; ++l) {
     // residual stream x (fp32) + its bf16 copy y + row sums of squares: ssA feeds QKV, ssB feeds FFN-up
-    bool ok = make_gemm_plan(&ws->qkv[l], VNB_EPI_QKV, ws->y.p, wqkv + l * 3 * dd, ws->M, 3 * d, d, ws->qk.p, ws->vT.p,
-                             nullptr, T, ws->Tpad, 2 * d) &&
-              make_gemm_plan(&ws->wo[l], VNB_EPI_RESID, ws->att.p, wo + l * dd, ws->M, d, d, ws->x.p, nullptr, nullptr, T,
-                             ws->Tpad, 0) &&
-              make_gemm_plan(&ws->up[l], VNB_EPI_GEGLU, ws->y.p, w1 + l * 4 * dd, ws->M, 4 * d, d, ws->h.p, nullptr,
-                             nullptr, T, ws->Tpad, 0) &&
-              make_gemm_plan(&ws->down[l], VNB_EPI_RESID, ws->h.p, w2 + l * 2 * dd, ws->M, d, 2 * d, ws->x.p, nullptr,
-                             nullptr, T, ws->Tpad, 0);
+    bool ok = plan(ws->qkv[l], VNB_EPI_QKV, ws->y.p, wqkv + l * 3 * dd, 3 * d, d, ws->qk.p, ws->vT.p, nullptr, &ws->ssA,
+                   nullptr) &&
+              plan(ws->wo[l], VNB_EPI_RESID, ws->att.p, wo + l * dd, d, d, ws->x.p, nullptr, nullptr, nullptr, &ws->ssB) &&
+              plan(ws->up[l], VNB_EPI_GEGLU, ws->y.p, w1 + l * 4 * dd, 4 * d, d, ws->h.p, nullptr, nullptr, &ws->ssB,
+                   nullptr) &&
+              plan(ws->down[l], VNB_EPI_RESID, ws->h.p, w2 + l * 2 * dd, d, 2 * d, ws->x.p, nullptr, nullptr, nullptr,
+                   &ws->ssA);
     if (!ok) return fail("plan layer %d: %s", l, tmap_error());
-    consumer(ws->qkv[l], ws->ssA);
-    consumer(ws->up[l], ws->ssB);
-    if (!producer(ws->wo[l], ws->ssB) || !producer(ws->down[l], ws->ssA)) return fail("plan layer %d: %s", l, tmap_error());
   }
-  if (!make_gemm_plan(&ws->cls, VNB_EPI_BIAS_F32, ws->y.p, m->w.wcls, ws->M, Cp * c.vocab_size, d, nullptr, nullptr,
-                      m->w.bcls, T, ws->Tpad, 0))
+  if (!plan(ws->cls, VNB_EPI_BIAS_F32, ws->y.p, m->w.wcls, Cp * c.vocab_size, d, nullptr, nullptr, m->w.bcls, &ws->ssA,
+            nullptr))
     return fail("plan classifier: %s", tmap_error());
-  consumer(ws->cls, ws->ssA);
   // generate loop: the same GEMM with the sampling epilogue; the logits are consumed in the epilogue and never stored
   ws->can_fuse = c.vocab_size % 128 == 0 && c.vocab_size <= 1024;
   if (ws->can_fuse) {
     CK(ws->partials.alloc(M * static_cast<size_t>(Cp) * (c.vocab_size / 128) * 16));
     ws->cls_sample = ws->cls;
-    ws->cls_sample.epi = VNB_EPI_SAMPLE;
-    ws->cls_sample.out = nullptr;
-    ws->cls_sample.zcur = ws->zcur.as<int32_t>();
-    ws->cls_sample.rowgrp = ws->rowgrp.as<RowGroup>();
-    ws->cls_sample.partials = ws->partials.p;
-    ws->cls_sample.C = c.n_codebooks; ws->cls_sample.ncc = c.n_conditioning_codebooks;
-    ws->cls_sample.V = c.vocab_size; ws->cls_sample.mask_token = c.vocab_size;
+    GemmArgs& s = ws->cls_sample.args;
+    s.epi = VNB_EPI_SAMPLE;
+    s.out = nullptr;
+    s.zcur = ws->zcur.as<int32_t>();
+    s.rowgrp = ws->rowgrp.as<RowGroup>();
+    s.partials = ws->partials.as<float4>();
+    s.C = c.n_codebooks; s.ncc = c.n_conditioning_codebooks; s.V = c.vocab_size; s.mask_token = c.vocab_size;
   }
   // embedding out_proj (layers.py:162) as a split-bf16 tensor-core contraction: x = A . emb_w3^T + bias, which also
   // emits bf16(x) and the row sums of squares the first QKV projection's fused RMSNorm consumes
-  if (!make_gemm_plan(&ws->emb, VNB_EPI_BIAS_F32, ws->embA.p, m->w.emb_w3, ws->M, d, 3 * ws->embKp, ws->x.p, nullptr,
-                      m->w.emb_b, T, ws->Tpad, 0) ||
-      !gemm_plan_set_fused_out(&ws->emb, ws->y.p, ws->ssA.as<float>()))
+  if (!plan(ws->emb, VNB_EPI_BIAS_F32, ws->embA.p, m->w.emb_w3, d, 3 * ws->embKp, ws->x.p, nullptr, m->w.emb_b, nullptr,
+            &ws->ssA))
     return fail("plan embedding: %s", tmap_error());
   if (!make_attn_plan(&ws->attn, ws->qk.p, ws->vT.p, ws->att.p, m->w.rel_bias, m->w.rel_sat, B, T, ws->Tpad, c.n_heads))
     return fail("plan attention: %s", tmap_error());
@@ -340,7 +342,7 @@ static int run_embed(vnb_model* m, Workspace* ws, const int32_t* codes_btc, cons
                                         c.vocab_size + 1, c.n_codebooks * 8, ws->embKp, ws->ssA.as<float>(),
                                         c.d_model / 256, ws->ss_parts, live, st));
   GemmPlan emb = ws->emb;
-  emb.live = live;
+  emb.args.live = live;
   LAUNCH(FAM_EMBED, launch_gemm(emb, st));
   return 0;
 }
@@ -353,62 +355,64 @@ static int run_lora_gemm(vnb_model* m, Workspace* ws, const GemmPlan& plan, int 
     return 0;
   }
   GemmPlan p = plan;  // carries the live bound of the iteration, which the down-projection shares
-  p.lora.table = m->adapter_tab.as<AdapterDev>();
-  p.lora.grp_adapter = ws->grp_adapter.as<int32_t>();
-  p.lora.rowgrp = ws->rowgrp.as<RowGroup>();
-  p.lora.rows_per_grp = ws->T;
-  p.lora.slot = slot;
-  p.lora.layer = l;
-  p.lora.u = ws->lora_u.as<float>();
-  LAUNCH(FAM_LORA_DOWN, launch_lora_down(a, p.M, p.K, p.lora, p.live, p.T, st));
+  AdapterRefs& r = p.args.lora;
+  r.table = m->adapter_tab.as<AdapterDev>();
+  r.grp_adapter = ws->grp_adapter.as<int32_t>();
+  r.rowgrp = ws->rowgrp.as<RowGroup>();
+  r.rows_per_grp = ws->T;
+  r.slot = slot;
+  r.layer = l;
+  r.u = ws->lora_u.as<float>();
+  LAUNCH(FAM_LORA_DOWN, launch_lora_down(a, p.args.M, p.args.K, r, p.args.live, p.args.T, st));
   LAUNCH(fam, launch_gemm(p, st));
   return 0;
 }
 
-// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  fused_dyn: the
-// classifier samples in its epilogue instead; with `logits` as well, the split epilogue stores the logits of the rows of
-// nucleus (top-p) groups there.  ragged: batch row b is a call of ws->frames[b] frames; its later frames are padding
-// that no earlier frame attends to.  live (device, null = every row): batch rows at or past live[0] are idle; every
-// kernel skips the tiles and CTAs wholly past them.
-static int run_stack(vnb_model* m, Workspace* ws, float* logits, cudaStream_t st, float* acts = nullptr,
-                     const SampleDyn* fused_dyn = nullptr, bool adapted = false, bool ragged = false,
-                     const int32_t* live = nullptr) {
+// x already holds the embedded input; runs the L layers + final norm + classifier into `logits`.  v.fused: the
+// classifier samples in its epilogue instead, from row `iter` of the ws->dyn table; with v.split as well, the split
+// epilogue stores the logits of the rows of nucleus (top-p) groups to `logits`.  v.ragged: batch row b is a call of
+// ws->frames[b] frames; its later frames are padding that no earlier frame attends to.  v.mixed_steps: batch rows at or
+// past ws->live[iter] are idle; every kernel skips the tiles and CTAs wholly past them.  acts (non-null): the residual
+// stream after every layer.
+static int run_stack(vnb_model* m, Workspace* ws, const Variant& v, int iter, float* logits, float* acts,
+                     cudaStream_t st) {
   const vnb_config& c = m->cfg;
   // RMSNorm (transformer.py:43-58) is fused: norm weights are folded into wqkv / w1 / wcls at pack time, the
   // producers of x (embed, attn-out, ffn-down) also emit bf16(x) and per-row sums of squares, and the consumers
   // scale their accumulator rows by rsqrt(mean(x^2) + eps).
-  const int32_t* frames = ragged ? ws->frames.as<int32_t>() : nullptr;
+  const int32_t* frames = v.ragged ? ws->frames.as<int32_t>() : nullptr;
+  const int32_t* live = v.mixed_steps ? ws->live.as<int32_t>() + iter : nullptr;
   AttnPlan attn = ws->attn;
   attn.frames = frames;
   attn.live = live;
   const auto bounded = [live](const GemmPlan& p) {
     GemmPlan q = p;
-    q.live = live;
+    q.args.live = live;
     return q;
   };
   for (int l = 0; l < c.n_layers; ++l) {
     GemmPlan qkv = bounded(ws->qkv[l]);
-    qkv.frames = frames;
-    if (run_lora_gemm(m, ws, qkv, FAM_GEMM_QKV, adapted, LORA_QKV, l, ws->y.p, st)) return 1;
+    qkv.args.frames = frames;
+    if (run_lora_gemm(m, ws, qkv, FAM_GEMM_QKV, v.adapted, LORA_QKV, l, ws->y.p, st)) return 1;
     LAUNCH(FAM_ATTN, launch_attention(attn, st));
-    if (run_lora_gemm(m, ws, bounded(ws->wo[l]), FAM_GEMM_O, adapted, LORA_WO, l, ws->att.p, st) ||
-        run_lora_gemm(m, ws, bounded(ws->up[l]), FAM_GEMM_UP, adapted, LORA_W1, l, ws->y.p, st) ||
-        run_lora_gemm(m, ws, bounded(ws->down[l]), FAM_GEMM_DOWN, adapted, LORA_W2, l, ws->h.p, st))
+    if (run_lora_gemm(m, ws, bounded(ws->wo[l]), FAM_GEMM_O, v.adapted, LORA_WO, l, ws->att.p, st) ||
+        run_lora_gemm(m, ws, bounded(ws->up[l]), FAM_GEMM_UP, v.adapted, LORA_W1, l, ws->y.p, st) ||
+        run_lora_gemm(m, ws, bounded(ws->down[l]), FAM_GEMM_DOWN, v.adapted, LORA_W2, l, ws->h.p, st))
       return 1;
     if (acts)  // return_activations: the residual stream after this layer (transformer.py:455-456)
       CK(cudaMemcpyAsync(acts + static_cast<size_t>(l) * ws->M * c.d_model, ws->x.p, ws->x.n, cudaMemcpyDeviceToDevice, st));
   }
-  if (fused_dyn != nullptr) {  // generate loop: sample in the classifier's epilogue, no logits tensor
+  if (v.fused) {  // generate loop: sample in the classifier's epilogue, no logits tensor
     GemmPlan cls = bounded(ws->cls_sample);
-    cls.dyn = fused_dyn;
-    if (logits != nullptr) {
-      cls.out = logits;
+    cls.args.dyn = ws->dyn.as<SampleDyn>() + static_cast<size_t>(iter) * ws->B;
+    if (v.split) {
+      cls.args.out = logits;
       cls.sample_split = true;
     }
     LAUNCH(FAM_GEMM_CLS, launch_gemm(cls, st));
   } else {
     GemmPlan cls = bounded(ws->cls);
-    cls.out = logits;
+    cls.args.out = logits;
     LAUNCH(FAM_GEMM_CLS, launch_gemm(cls, st));
   }
   m->prof.mark(-1, st);
@@ -457,6 +461,41 @@ static int one_group_rows(int rows, const RowGroup** out) {
   }
   *out = buf_dev[dev];
   return 0;
+}
+
+// The sampling scalars of one group at one step, as the sampling kernels read them.
+static SampleDyn sample_dyn(const vnb_sample_group& q) {
+  return SampleDyn{inv_temperature(q.temperature), q.gamma, q.temp_eff, q.do_sample, q.is_last, q.step, q.seed_lo,
+                   q.seed_hi, q.top_p};
+}
+
+// The groups of a launch of B batch rows (vnb_gen_group or vnb_sample_group): 1..B groups of >= 1 rows each, B in all.
+template <class Group>
+static int check_groups(const Group* groups, int n_groups, int B, const char* who) {
+  if (n_groups < 1 || n_groups > B) return fail("%s: n_groups %d out of range 1..B (B = %d)", who, n_groups, B);
+  long long total = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    if (groups[g].rows < 1) return fail("%s: group %d has %d rows", who, g, groups[g].rows);
+    total += groups[g].rows;
+  }
+  if (total != B) return fail("%s: group rows sum to %lld, not B = %d", who, total, B);
+  return 0;
+}
+
+// The row -> group map of checked groups: group g holds the groups[g].rows batch rows that follow group g - 1's.
+template <class Group>
+static std::vector<RowGroup> row_groups(const Group* groups, int n_groups, int B) {
+  std::vector<RowGroup> rowgrp(B);
+  for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g)
+    for (int b = first; b < first + groups[g].rows; ++b) rowgrp[b] = RowGroup{g, first};
+  return rowgrp;
+}
+
+static AdapterDev adapter_dev(const vnb_adapter_weights& w) {
+  const float* ptrs[2 * LORA_SLOTS] = {w.a_qkv, w.b_qkv, w.a_wo, w.b_wo, w.a_w1, w.b_w1, w.a_w2, w.b_w2};
+  AdapterDev a;
+  for (int s = 0; s < LORA_SLOTS; ++s) { a.a[s] = ptrs[2 * s]; a.b[s] = ptrs[2 * s + 1]; }
+  return a;
 }
 
 // Adapter ids of a launch (host, n entries; NULL = none): each -1 or a live id.
@@ -518,16 +557,15 @@ int32_t vnb_model_create(const vnb_config* cfg, const vnb_weights* w, vnb_model*
 
 int32_t vnb_adapter_add(vnb_model* m, const vnb_adapter_weights* w, int32_t* id) {
   if (!m || !w || !id) return fail("vnb_adapter_add: null argument");
-  const float* ptrs[2 * LORA_SLOTS] = {w->a_qkv, w->b_qkv, w->a_wo, w->b_wo, w->a_w1, w->b_w1, w->a_w2, w->b_w2};
+  const AdapterDev a = adapter_dev(*w);
   static const char* names[2 * LORA_SLOTS] = {"a_qkv", "b_qkv", "a_wo", "b_wo", "a_w1", "b_w1", "a_w2", "b_w2"};
   for (int i = 0; i < 2 * LORA_SLOTS; ++i)
-    if (!ptrs[i]) return fail("vnb_adapter_add: %s is NULL", names[i]);
+    if (!(i % 2 ? a.b[i / 2] : a.a[i / 2])) return fail("vnb_adapter_add: %s is NULL", names[i]);
   int slot = -1;
   for (int i = 0; i < VNB_MAX_ADAPTERS && slot < 0; ++i)
     if (!m->adapter_live[i]) slot = i;
   if (slot < 0) return fail("vnb_adapter_add: the adapter table is full (%d live adapters)", VNB_MAX_ADAPTERS);
-  AdapterDev& a = m->adapters[slot];
-  for (int s = 0; s < LORA_SLOTS; ++s) { a.a[s] = ptrs[2 * s]; a.b[s] = ptrs[2 * s + 1]; }
+  m->adapters[slot] = a;
   m->adapter_live[slot] = true;
   *id = slot;
   return 0;
@@ -564,7 +602,9 @@ int32_t vnb_forward_codes_adapted(vnb_model* m, const int64_t* codes, int32_t B,
                                     nullptr, 1, B, c.n_codebooks, T, /*ncc=*/c.n_codebooks, c.vocab_size, st));
   if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st)) return 1;
   m->last = ws;
-  return run_stack(m, ws, logits, st, nullptr, nullptr, adapted);
+  Variant v;
+  v.adapted = adapted;
+  return run_stack(m, ws, v, 0, logits, nullptr, st);
 }
 
 int32_t vnb_forward_codes(vnb_model* m, const int64_t* codes, int32_t B, int32_t T, float* logits, void* stream) {
@@ -577,7 +617,7 @@ int32_t vnb_forward_latents(vnb_model* m, const float* latents, int32_t B, int32
   if (get_workspace(m, B, T, &ws)) return 1;
   if (run_embed(m, ws, nullptr, latents, st)) return 1;
   m->last = ws;
-  return run_stack(m, ws, logits, st);
+  return run_stack(m, ws, Variant{}, 0, logits, nullptr, st);
 }
 
 int32_t vnb_forward_latents_acts(vnb_model* m, const float* latents, int32_t B, int32_t T, float* logits, float* acts,
@@ -587,7 +627,7 @@ int32_t vnb_forward_latents_acts(vnb_model* m, const float* latents, int32_t B, 
   if (get_workspace(m, B, T, &ws)) return 1;
   if (run_embed(m, ws, nullptr, latents, st)) return 1;
   m->last = ws;
-  return run_stack(m, ws, logits, st, acts);
+  return run_stack(m, ws, Variant{}, 0, logits, acts, st);
 }
 
 int32_t vnb_get_hidden(vnb_model* m, float* out, void* stream) {
@@ -608,12 +648,13 @@ static int fused_sampler_enabled() {
   return g_fused_sampler;
 }
 
-// mixed_steps: iteration i runs only the batch rows ws->live[i] counts (a prefix); the others are idle and untouched.
-// split (with fused): nucleus and plain groups; the classifier stores the nucleus rows' logits, and the sampler runs the
-// combine for the plain rows and the nucleus draw for the others.
-static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int steps, int64_t* out,
-                            cudaStream_t st, bool use_top_p, bool fused, bool adapted, bool ragged, bool mixed_steps,
-                            bool split) {
+}  // extern "C"
+
+// v.mixed_steps: iteration i runs only the batch rows ws->live[i] counts (a prefix); the others are idle and untouched.
+// v.split (with v.fused): nucleus and plain groups; the classifier stores the nucleus rows' logits, and the sampler runs
+// the combine for the plain rows and the nucleus draw for the others.
+static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const int32_t* mask, int64_t* out,
+                            const Variant& v, cudaStream_t st) {
   const vnb_config& c = m->cfg;
   const int ncc = c.n_conditioning_codebooks;
   // the whole n0 array is zeroed (a captured graph replays with any number of groups up to B)
@@ -628,21 +669,18 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   sa.n0 = ws->n0.as<int32_t>();
   sa.rowgrp = ws->rowgrp.as<RowGroup>();
   sa.B = ws->B; sa.T = ws->T; sa.C = c.n_codebooks; sa.ncc = ncc; sa.V = c.vocab_size; sa.mask_token = c.vocab_size;
-  for (int i = 0; i < steps; ++i) {
-    const int32_t* live = mixed_steps ? ws->live.as<int32_t>() + i : nullptr;
-    sa.live = live;
-    if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st, live)) return 1;
+  for (int i = 0; i < v.steps; ++i) {
+    sa.live = v.mixed_steps ? ws->live.as<int32_t>() + i : nullptr;
+    if (run_embed(m, ws, ws->zcur.as<int32_t>(), nullptr, st, sa.live)) return 1;
+    if (run_stack(m, ws, v, i, ws->logits.as<float>(), nullptr, st)) return 1;
     const SampleDyn* dyn_i = ws->dyn.as<SampleDyn>() + static_cast<size_t>(i) * ws->B;
-    if (split) {
-      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, dyn_i, adapted, ragged, live)) return 1;
+    if (v.split) {
       LAUNCH(FAM_SAMPLE, launch_sample_split_dev(sa, ws->partials.p, dyn_i, st));
       ++g_launches;  // the split sampler is one kernel more
-    } else if (fused) {
-      if (run_stack(m, ws, nullptr, st, nullptr, dyn_i, adapted, ragged, live)) return 1;
+    } else if (v.fused) {
       LAUNCH(FAM_SAMPLE, launch_sample_combine_dev(sa, ws->partials.p, dyn_i, st));
     } else {
-      if (run_stack(m, ws, ws->logits.as<float>(), st, nullptr, nullptr, adapted, ragged, live)) return 1;
-      LAUNCH(FAM_SAMPLE, launch_sample_step_dev(sa, dyn_i, st, use_top_p));
+      LAUNCH(FAM_SAMPLE, launch_sample_step_dev(sa, dyn_i, st, v.top_p));
     }
     ++g_launches;  // sample step = two kernels
   }
@@ -651,109 +689,129 @@ static int enqueue_generate(vnb_model* m, Workspace* ws, const int64_t* z, const
   return 0;
 }
 
-}  // extern "C"
+// One generate launch as a vnb_generate* entry point describes it.  Group g runs steps_g steps with its own gamma
+// schedule: group_steps[g] and group_gamma[g] from the entry points that take them (per_group), else every group runs
+// `steps` with `gamma`.
+struct GenDesc {
+  const char* who;  // the entry point called, named in refusals
+  const int64_t* z;
+  const int32_t* mask;
+  int B, T;
+  const vnb_gen_group* groups;
+  int n_groups, use_graph;
+  int64_t* out;
+  int steps = 0;
+  const float* gamma = nullptr;
+  bool per_group = false;
+  const int32_t* group_steps = nullptr;
+  const float* const* group_gamma = nullptr;
+  const int32_t* group_frames = nullptr;   // null: every group has T frames
+  const int32_t* group_adapter = nullptr;  // null: no group is adapted
+  bool mixed_top_p = false;  // groups may mix nucleus (top-p) and plain sampling
+};
 
-// The launch behind vnb_generate_ragged, vnb_generate_steps and vnb_generate_mixed_top_p: group g runs group_steps[g]
-// steps (NULL: every group runs `steps`) with its own gamma schedule group_gamma[g] (NULL: every group uses `gamma`).
-// The caller has checked the steps and their order; `steps` is their maximum S.  Group g is idle for the first
-// S - steps_g iterations and then runs its own step j = i - (S - steps_g) with j's schedule values, Philox step word and
-// last-step flag.  mixed_top_p: groups may mix nucleus (top-p) and plain sampling, each row drawing as its group's own
-// launch would.
-static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
-                           const float* gamma, const int32_t* group_steps, const float* const* group_gamma,
-                           const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
-                           const int32_t* group_adapter, int32_t use_graph, int64_t* out, cudaStream_t st,
-                           bool mixed_top_p = false) {
-  if (steps < 1 || steps > vnb_model::kMaxSteps) return fail("bad sampling_steps %d (1..%d)", steps, vnb_model::kMaxSteps);
-  if ((!gamma && !group_gamma) || !groups) return fail("vnb_generate_many: gamma and groups are required");
-  if (B < 1 || T < 1) return fail("vnb_generate_many: need B >= 1 and T >= 1 (got %d, %d)", B, T);
-  if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
+// Every refusal of a generate launch, required pointers first.  Fills what the description decides of the launch's
+// variant: v->steps = S, the most steps of any group; *top_p_mix: groups mix nucleus and plain sampling.
+static int check_generate(const vnb_model* m, const GenDesc& d, Variant* v, bool* top_p_mix) {
+  constexpr int kMax = vnb_model::kMaxSteps;
+  if (d.per_group ? (!d.group_steps || !d.group_gamma || !d.groups) : (!d.gamma || !d.groups))
+    return fail("%s: %s are required", d.who, d.per_group ? "group_steps, group_gamma and groups" : "gamma and groups");
+  if (d.B < 1 || d.T < 1) return fail("%s: need B >= 1 and T >= 1 (got %d, %d)", d.who, d.B, d.T);
+  if (check_groups(d.groups, d.n_groups, d.B, d.who)) return 1;
+  if (!d.per_group && (d.steps < 1 || d.steps > kMax)) return fail("%s: bad sampling_steps %d (1..%d)", d.who, d.steps, kMax);
   const auto top_p_on = [](float tp) { return tp > 0.f && tp < 1.f; };
-  bool use_top_p = top_p_on(groups[0].top_p), top_p_mix = false;
-  long long total = 0;
-  for (int g = 0; g < n_groups; ++g) {
-    const vnb_gen_group& q = groups[g];
-    if (q.rows < 1) return fail("vnb_generate_many: group %d has %d rows", g, q.rows);
-    if (!q.temp_eff || !q.do_sample) return fail("vnb_generate_many: group %d lacks its schedules", g);
+  v->steps = d.per_group ? d.group_steps[0] : d.steps;
+  v->has_mask = d.mask != nullptr;
+  v->top_p = top_p_on(d.groups[0].top_p);
+  for (int g = 0; g < d.n_groups; ++g) {
+    const vnb_gen_group& q = d.groups[g];
+    if (d.per_group) {
+      const int n = d.group_steps[g];
+      if (n < 1 || n > kMax) return fail("%s: group %d has %d sampling steps, outside 1..%d", d.who, g, n, kMax);
+      // longest first: the live rows of every iteration are then a prefix of the batch
+      if (g > 0 && n > d.group_steps[g - 1])
+        return fail("%s: group %d has %d steps, more than group %d's %d (the order must be non-increasing)", d.who, g,
+                    n, g - 1, d.group_steps[g - 1]);
+      if (!d.group_gamma[g]) return fail("%s: group %d lacks its schedules (gamma)", d.who, g);
+      v->mixed_steps |= n != v->steps;
+    }
+    if (!q.temp_eff || !q.do_sample) return fail("%s: group %d lacks its schedules", d.who, g);
     // outside vnb_generate_mixed_top_p the sampler variant is chosen per launch: a mixed launch would filter
     // differently from the separate calls
-    if (top_p_on(q.top_p) != top_p_on(groups[0].top_p)) {
-      if (!mixed_top_p) return fail("vnb_generate_many: groups mix top-p and no top-p sampling");
-      top_p_mix = true;
-      use_top_p = true;
+    if (top_p_on(q.top_p) != top_p_on(d.groups[0].top_p)) {
+      if (!d.mixed_top_p) return fail("%s: groups mix top-p and no top-p sampling", d.who);
+      *top_p_mix = true;
+      v->top_p = true;
     }
-    total += q.rows;
-  }
-  if (total != B) return fail("vnb_generate_many: group rows sum to %lld, not B = %d", total, B);
-  // a group shorter than T: its rows' later frames are padding (kept frames in z / mask) that attention never reads
-  bool ragged = false;
-  for (int g = 0; group_frames && g < n_groups; ++g) {
-    if (group_frames[g] < 1 || group_frames[g] > T)
-      return fail("vnb_generate_ragged: group %d has %d frames, outside 1..T (T = %d)", g, group_frames[g], T);
-    ragged |= group_frames[g] < T;
+    // a group shorter than T: its rows' later frames are padding (kept frames in z / mask) that attention never reads
+    if (d.group_frames && (d.group_frames[g] < 1 || d.group_frames[g] > d.T))
+      return fail("%s: group %d has %d frames, outside 1..T (T = %d)", d.who, g, d.group_frames[g], d.T);
+    v->ragged |= d.group_frames && d.group_frames[g] < d.T;
   }
   // without a mask every predicted codebook is masked, padding included: it would be sampled and count in N0
-  if (ragged && !mask) return fail("vnb_generate_ragged: a launch with groups shorter than T needs a mask");
-  if (check_adapter_ids(m, group_adapter, n_groups, "vnb_generate_many_adapted")) return 1;
-  const bool adapted = any_adapted(group_adapter, n_groups);
-  bool mixed_steps = false;
-  for (int g = 0; group_steps && g < n_groups; ++g) mixed_steps |= group_steps[g] != steps;
+  if (v->ragged && !d.mask) return fail("%s: a launch with groups shorter than T needs a mask", d.who);
+  if (check_adapter_ids(m, d.group_adapter, d.n_groups, d.who)) return 1;
+  v->adapted = any_adapted(d.group_adapter, d.n_groups);
+  return 0;
+}
+
+// The launch behind every vnb_generate* entry point.  Group g is idle for the first S - steps_g iterations and then runs
+// its own step j = i - (S - steps_g) with j's schedule values, Philox step word and last-step flag.  With mixed_top_p,
+// each row draws as its group's own launch would.
+static int generate(vnb_model* m, const GenDesc& d, void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  Variant v;
+  bool top_p_mix = false;
+  if (check_generate(m, d, &v, &top_p_mix)) return 1;
+  const int B = d.B, S = v.steps;
   Workspace* ws;
-  if (get_workspace(m, B, T, &ws)) return 1;
+  if (get_workspace(m, B, d.T, &ws)) return 1;
   m->last = ws;
-  // the [step][group] table (row stride B), the row map and the live rows per iteration, pageable sources: the runtime
-  // stages them before returning, so the vectors may die at scope exit
-  std::vector<SampleDyn> dyn(static_cast<size_t>(steps) * B);
-  std::vector<RowGroup> rowgrp(B);
-  std::vector<int32_t> frames(ragged ? B : 0);
-  std::vector<int32_t> live(mixed_steps ? steps : 0, 0);
-  for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
-    const vnb_gen_group& q = groups[g];
-    const float inv_t = inv_temperature(q.temperature);
-    const int steps_g = group_steps ? group_steps[g] : steps;
-    const float* gam = group_gamma ? group_gamma[g] : gamma;
-    const int idle = steps - steps_g;  // iterations before the group's first step
-    for (int i = 0; i < steps; ++i) {
-      SampleDyn& d = dyn[static_cast<size_t>(i) * B + g];
-      d = SampleDyn{};
-      d.inv_temp = inv_t;
-      d.seed_lo = q.seed_lo;
-      d.seed_hi = q.seed_hi;
-      d.top_p = q.top_p;
-      if (i < idle) continue;  // no kernel reads an idle group's entry
-      const int j = i - idle;
-      d.gamma = gam[j];
-      d.temp_eff = q.temp_eff[j];
-      d.do_sample = q.do_sample[j];
-      d.is_last = (j == steps_g - 1);
-      d.step = j;
-      if (mixed_steps) live[i] += q.rows;
+  // the [step][group] table (row stride B), the row map, the frames and the live rows per iteration, pageable sources:
+  // the runtime stages them before returning, so the vectors may die at scope exit
+  std::vector<SampleDyn> dyn(static_cast<size_t>(S) * B);
+  const std::vector<RowGroup> rowgrp = row_groups(d.groups, d.n_groups, B);
+  std::vector<int32_t> frames(v.ragged ? B : 0);
+  std::vector<int32_t> live(v.mixed_steps ? S : 0, 0);
+  for (int g = 0; g < d.n_groups; ++g) {
+    const vnb_gen_group& q = d.groups[g];
+    const int steps_g = d.per_group ? d.group_steps[g] : S;
+    const float* gam = d.per_group ? d.group_gamma[g] : d.gamma;
+    const int idle = S - steps_g;  // iterations before the group's first step
+    vnb_sample_group s = {};  // an idle group's entry: no kernel reads more than its temperature, seeds and top-p
+    s.temperature = q.temperature; s.seed_lo = q.seed_lo; s.seed_hi = q.seed_hi; s.top_p = q.top_p;
+    for (int i = 0; i < S; ++i) {
+      if (i >= idle) {
+        const int j = i - idle;
+        s.gamma = gam[j]; s.temp_eff = q.temp_eff[j]; s.do_sample = q.do_sample[j]; s.is_last = j == steps_g - 1;
+        s.step = j;
+        if (v.mixed_steps) live[i] += q.rows;
+      }
+      dyn[static_cast<size_t>(i) * B + g] = sample_dyn(s);
     }
-    for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
-    for (int b = first; ragged && b < first + q.rows; ++b) frames[b] = group_frames[g];
   }
+  for (int b = 0; v.ragged && b < B; ++b) frames[b] = d.group_frames[rowgrp[b].group];
   CK(cudaMemcpyAsync(ws->dyn.p, dyn.data(), sizeof(SampleDyn) * dyn.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(ws->rowgrp.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
-  if (ragged) CK(cudaMemcpyAsync(ws->frames.p, frames.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
-  if (mixed_steps) CK(cudaMemcpyAsync(ws->live.p, live.data(), sizeof(int32_t) * steps, cudaMemcpyHostToDevice, st));
-  if (adapted && stage_adapters(m, ws, group_adapter, n_groups, st)) return 1;
+  if (v.ragged) CK(cudaMemcpyAsync(ws->frames.p, frames.data(), sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
+  if (v.mixed_steps) CK(cudaMemcpyAsync(ws->live.p, live.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+  if (v.adapted && stage_adapters(m, ws, d.group_adapter, d.n_groups, st)) return 1;
   // a mix of nucleus and plain groups: the split path when the sampler is fused, else the materialising path with the
   // nucleus kernel for every row (a group whose top-p is off draws there as without the filter, bit for bit)
-  const bool split = top_p_mix && fused_sampler_enabled() != 0 && ws->can_fuse;
-  const bool fused = fused_sampler_enabled() != 0 && (!use_top_p || split) && ws->can_fuse;
-  if ((!fused || split) && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
+  v.split = top_p_mix && fused_sampler_enabled() != 0 && ws->can_fuse;
+  v.fused = fused_sampler_enabled() != 0 && (!v.top_p || v.split) && ws->can_fuse;
+  v.gemm_pair = get_gemm_pair();
+  if ((!v.fused || v.split) && ws->logits.p == nullptr)  // before any capture: cudaMalloc is not capturable
     CK(ws->logits.alloc(static_cast<size_t>(ws->M) * (m->cfg.n_codebooks - m->cfg.n_conditioning_codebooks) * m->cfg.vocab_size * 4));
-  if (!use_graph || m->prof.on)
-    return enqueue_generate(m, ws, z, mask, steps, out, st, use_top_p, fused, adapted, ragged, mixed_steps, split);
+  if (!d.use_graph || m->prof.on) return enqueue_generate(m, ws, d.z, d.mask, d.out, v, st);
 
-  const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * T;
-  CK(cudaMemcpyAsync(ws->z_in.p, z, nz * 8, cudaMemcpyDeviceToDevice, st));
-  if (mask) CK(cudaMemcpyAsync(ws->mask_in.p, mask, nz * 4, cudaMemcpyDeviceToDevice, st));
+  const size_t nz = static_cast<size_t>(B) * m->cfg.n_codebooks * d.T;
+  CK(cudaMemcpyAsync(ws->z_in.p, d.z, nz * 8, cudaMemcpyDeviceToDevice, st));
+  if (d.mask) CK(cudaMemcpyAsync(ws->mask_in.p, d.mask, nz * 4, cudaMemcpyDeviceToDevice, st));
   const int64_t* gz = ws->z_in.as<int64_t>();
-  const int32_t* gmask = mask ? ws->mask_in.as<int32_t>() : nullptr;
+  const int32_t* gmask = d.mask ? ws->mask_in.as<int32_t>() : nullptr;
   int64_t* gout = ws->z_out.as<int64_t>();
-  GraphKey key{steps, mask != nullptr, use_top_p, get_gemm_pair(), fused, adapted, ragged, mixed_steps, split};
-  auto it = ws->graphs.find(key);
+  auto it = ws->graphs.find(v);
   if (it == ws->graphs.end()) {
     cudaStream_t cap;
     CK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
@@ -761,7 +819,7 @@ static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, 
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) { cudaStreamDestroy(cap); return fail("begin capture: %s", cudaGetErrorString(e)); }
     const unsigned long long before = g_launches;
-    int rc = enqueue_generate(m, ws, gz, gmask, steps, gout, cap, use_top_p, fused, adapted, ragged, mixed_steps, split);
+    int rc = enqueue_generate(m, ws, gz, gmask, gout, v, cap);
     const unsigned long long in_graph = g_launches - before;
     g_launches = before;
     e = cudaStreamEndCapture(cap, &graph);
@@ -777,89 +835,72 @@ static int generate_launch(vnb_model* m, const int64_t* z, const int32_t* mask, 
       ws->graphs.clear();
       ws->graph_kernels.clear();
     }
-    it = ws->graphs.emplace(key, exec).first;
+    it = ws->graphs.emplace(v, exec).first;
     ++g_captures;
-    ws->graph_kernels[key] = in_graph;
+    ws->graph_kernels[v] = in_graph;
   }
   CK(cudaGraphLaunch(it->second, st));
-  g_launches += ws->graph_kernels[key];
-  CK(cudaMemcpyAsync(out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
+  g_launches += ws->graph_kernels[v];
+  CK(cudaMemcpyAsync(d.out, ws->z_out.p, nz * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
 extern "C" {
 
+// One call is the one-group launch.
+int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                     const vnb_gen_params* p, int64_t* out, void* stream) {
+  if (!p) return fail("vnb_generate: the parameters are required");
+  vnb_gen_group g;
+  g.rows = B; g.temperature = p->temperature; g.temp_eff = p->temp_eff; g.do_sample = p->do_sample;
+  g.seed_lo = p->seed_lo; g.seed_hi = p->seed_hi; g.top_p = p->top_p;
+  return generate(m, GenDesc{"vnb_generate", z, mask, B, T, &g, 1, p->use_graph, out, p->sampling_steps, p->gamma},
+                  stream);
+}
+
+int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
+                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
+                          int64_t* out, void* stream) {
+  return generate(m, GenDesc{"vnb_generate_many", z, mask, B, T, groups, n_groups, use_graph, out, steps, gamma},
+                  stream);
+}
+
+int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
+                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
+                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
+  GenDesc d{"vnb_generate_many_adapted", z, mask, B, T, groups, n_groups, use_graph, out, steps, gamma};
+  d.group_adapter = group_adapter;
+  return generate(m, d, stream);
+}
+
 int32_t vnb_generate_ragged(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
                             const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
                             const int32_t* group_frames, const int32_t* group_adapter, int32_t use_graph, int64_t* out,
                             void* stream) {
-  return generate_launch(m, z, mask, B, T, steps, gamma, nullptr, nullptr, groups, n_groups, group_frames,
-                         group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream));
+  GenDesc d{"vnb_generate_ragged", z, mask, B, T, groups, n_groups, use_graph, out, steps, gamma};
+  d.group_frames = group_frames; d.group_adapter = group_adapter;
+  return generate(m, d, stream);
 }
-
-}  // extern "C"
-
-// vnb_generate_steps, and with mixed_top_p vnb_generate_mixed_top_p
-static int generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                          const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
-                          int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
-                          int32_t use_graph, int64_t* out, void* stream, bool mixed_top_p) {
-  if (!group_steps || !group_gamma || !groups) return fail("vnb_generate_steps: group_steps, group_gamma and groups are required");
-  if (n_groups < 1 || n_groups > B) return fail("vnb_generate_many: n_groups %d out of range 1..B (B = %d)", n_groups, B);
-  for (int g = 0; g < n_groups; ++g) {
-    if (group_steps[g] < 1 || group_steps[g] > vnb_model::kMaxSteps)
-      return fail("vnb_generate_steps: group %d has %d sampling steps, outside 1..%d", g, group_steps[g],
-                  vnb_model::kMaxSteps);
-    // longest first: the live rows of every iteration are then a prefix of the batch
-    if (g > 0 && group_steps[g] > group_steps[g - 1])
-      return fail("vnb_generate_steps: group %d has %d steps, more than group %d's %d (the order must be non-increasing)",
-                  g, group_steps[g], g - 1, group_steps[g - 1]);
-    if (!group_gamma[g]) return fail("vnb_generate_steps: group %d lacks its schedules (gamma)", g);
-  }
-  return generate_launch(m, z, mask, B, T, group_steps[0], nullptr, group_steps, group_gamma, groups, n_groups,
-                         group_frames, group_adapter, use_graph, out, reinterpret_cast<cudaStream_t>(stream), mixed_top_p);
-}
-
-extern "C" {
 
 int32_t vnb_generate_steps(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
                            const int32_t* group_steps, const float* const* group_gamma, const vnb_gen_group* groups,
                            int32_t n_groups, const int32_t* group_frames, const int32_t* group_adapter,
                            int32_t use_graph, int64_t* out, void* stream) {
-  return generate_steps(m, z, mask, B, T, group_steps, group_gamma, groups, n_groups, group_frames, group_adapter,
-                        use_graph, out, stream, false);
+  GenDesc d{"vnb_generate_steps", z, mask, B, T, groups, n_groups, use_graph, out};
+  d.per_group = true; d.group_steps = group_steps; d.group_gamma = group_gamma;
+  d.group_frames = group_frames; d.group_adapter = group_adapter;
+  return generate(m, d, stream);
 }
 
 int32_t vnb_generate_mixed_top_p(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
                                  const int32_t* group_steps, const float* const* group_gamma,
                                  const vnb_gen_group* groups, int32_t n_groups, const int32_t* group_frames,
                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
-  return generate_steps(m, z, mask, B, T, group_steps, group_gamma, groups, n_groups, group_frames, group_adapter,
-                        use_graph, out, stream, true);
-}
-
-// Calls of one length are the group_frames = NULL case.
-int32_t vnb_generate_many_adapted(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                                  int32_t steps, const float* gamma, const vnb_gen_group* groups, int32_t n_groups,
-                                  const int32_t* group_adapter, int32_t use_graph, int64_t* out, void* stream) {
-  return vnb_generate_ragged(m, z, mask, B, T, steps, gamma, groups, n_groups, nullptr, group_adapter, use_graph, out,
-                             stream);
-}
-
-int32_t vnb_generate_many(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T, int32_t steps,
-                          const float* gamma, const vnb_gen_group* groups, int32_t n_groups, int32_t use_graph,
-                          int64_t* out, void* stream) {
-  return vnb_generate_many_adapted(m, z, mask, B, T, steps, gamma, groups, n_groups, nullptr, use_graph, out, stream);
-}
-
-// One call is the one-group launch.
-int32_t vnb_generate(vnb_model* m, const int64_t* z, const int32_t* mask, int32_t B, int32_t T,
-                     const vnb_gen_params* p, int64_t* out, void* stream) {
-  if (!p) return fail("bad sampling_steps");
-  vnb_gen_group g;
-  g.rows = B; g.temperature = p->temperature; g.temp_eff = p->temp_eff; g.do_sample = p->do_sample;
-  g.seed_lo = p->seed_lo; g.seed_hi = p->seed_hi; g.top_p = p->top_p;
-  return vnb_generate_many(m, z, mask, B, T, p->sampling_steps, p->gamma, &g, 1, p->use_graph, out, stream);
+  GenDesc d{"vnb_generate_mixed_top_p", z, mask, B, T, groups, n_groups, use_graph, out};
+  d.per_group = true; d.group_steps = group_steps; d.group_gamma = group_gamma;
+  d.group_frames = group_frames; d.group_adapter = group_adapter;
+  d.mixed_top_p = true;
+  return generate(m, d, stream);
 }
 
 uint64_t vnb_launch_count(void) { return g_launches; }
@@ -920,13 +961,12 @@ int32_t vnb_sample_step(const float* logits, int32_t* zflat, int32_t* tokens_out
                         int32_t do_sample, float temperature, float gamma, float temp_eff, uint32_t seed_lo,
                         uint32_t seed_hi, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  SampleDyn d;
-  d.inv_temp = inv_temperature(temperature);
-  d.gamma = gamma; d.temp_eff = temp_eff; d.do_sample = do_sample; d.is_last = is_last; d.step = step;
-  d.seed_lo = seed_lo; d.seed_hi = seed_hi; d.top_p = 0.f;
+  vnb_sample_group q = {};
+  q.temperature = temperature; q.gamma = gamma; q.temp_eff = temp_eff; q.do_sample = do_sample; q.is_last = is_last;
+  q.step = step; q.seed_lo = seed_lo; q.seed_hi = seed_hi;
   const SampleDyn* dd = nullptr;
   const RowGroup* rg = nullptr;
-  if (stage_sample_dyn(d, st, &dd) || one_group_rows(B, &rg)) return 1;
+  if (stage_sample_dyn(sample_dyn(q), st, &dd) || one_group_rows(B, &rg)) return 1;
   SampleArgs sa;
   sa.logits = logits; sa.zcur = zflat; sa.zorig = nullptr; sa.tokens = tokens_out; sa.conf = conf_out; sa.n0 = n0;
   sa.rowgrp = rg;
@@ -942,12 +982,88 @@ int32_t vnb_dbg_set_live(const int32_t* live) {
   g_dbg_live = live;
   return 0;
 }
+}  // extern "C"
+
+// The plan of a unit-level GEMM entry point: built by make_gemm_plan as get_workspace() builds the forward's, so the
+// tests reach every epilogue branch the forward launches, and bounded by vnb_dbg_set_live.  Refuses what no forward
+// plan is: fused-norm operands and QKV shapes the epilogues cannot take.
+static int unit_gemm_plan(GemmPlan* p, const char* who, int epi, const void* A, const void* W, int M, int N, int K,
+                          void* out, void* out2, const float* bias, int T, int Tpad, const float* ss_in, int ss_parts,
+                          float inv_d, float eps, void* out_bf16, float* ss_out) {
+  if ((out_bf16 != nullptr || ss_out != nullptr) && epi != VNB_EPI_RESID && epi != VNB_EPI_BIAS_F32)
+    return fail("%s: out_bf16 / ss_out need the RESID or BIAS_F32 epilogue", who);
+  if ((out_bf16 == nullptr) != (ss_out == nullptr)) return fail("%s: out_bf16 and ss_out go together", who);
+  if (ss_in != nullptr && ss_parts < 1) return fail("%s: ss_parts must be >= 1", who);
+  if (epi == VNB_EPI_QKV && (out2 == nullptr || N % 96 != 0 || T < 1 || Tpad < T))
+    return fail("%s: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad", who);
+  if (!make_gemm_plan(p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, ss_in, ss_parts, inv_d, eps, out_bf16, ss_out))
+    return fail("gemm plan: %s", tmap_error());
+  p->args.live = g_dbg_live;
+  return 0;
+}
+
+// vnb_dbg_gemm_adapted, and (frames non-null) the adapted QKV of vnb_dbg_gemm_qkv_frames
+static int dbg_gemm_adapted(const char* who, int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K,
+                            void* out, void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts,
+                            float inv_d, float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
+                            int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u,
+                            const int32_t* frames, void* stream) {
+  if (epi != VNB_EPI_QKV && epi != VNB_EPI_RESID && epi != VNB_EPI_GEGLU)
+    return fail("%s: epilogue %d has no adapted variant", who, epi);
+  if (!adapters || n_adapters < 1 || n_adapters > VNB_MAX_ADAPTERS || !row_adapter || !u || layer < 0)
+    return fail("%s: need 1..%d adapters, a row map, u and layer >= 0", who, VNB_MAX_ADAPTERS);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  std::vector<AdapterDev> tab(VNB_MAX_ADAPTERS);
+  for (int i = 0; i < n_adapters; ++i) tab[i] = adapter_dev(adapters[i]);
+  std::vector<RowGroup> rowgrp(M);
+  for (int i = 0; i < M; ++i) rowgrp[i] = RowGroup{i, i};  // row m is its own group: grp_adapter = row_adapter
+  GemmPlan p;
+  if (unit_gemm_plan(&p, who, epi, A, W, M, N, K, out, out2, nullptr, T, Tpad, ss_in, ss_parts, inv_d, eps, out_bf16,
+                     ss_out))
+    return 1;
+  DevBuf tab_dev, grp_dev;
+  CK(tab_dev.alloc(sizeof(AdapterDev) * VNB_MAX_ADAPTERS));
+  CK(grp_dev.alloc(sizeof(RowGroup) * M));
+  CK(cudaMemcpyAsync(tab_dev.p, tab.data(), sizeof(AdapterDev) * VNB_MAX_ADAPTERS, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * M, cudaMemcpyHostToDevice, st));
+  AdapterRefs& r = p.args.lora;
+  r.table = tab_dev.as<AdapterDev>();
+  r.grp_adapter = row_adapter;
+  r.rowgrp = grp_dev.as<RowGroup>();
+  r.rows_per_grp = 1;
+  r.slot = epi == VNB_EPI_QKV ? LORA_QKV : epi == VNB_EPI_GEGLU ? LORA_W1 : (K == N ? LORA_WO : LORA_W2);
+  r.layer = layer;
+  r.u = u;
+  p.args.frames = frames;
+  CK(launch_lora_down(A, M, K, r, p.args.live, T, st));
+  CK(launch_gemm(p, st));
+  CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
+  return 0;
+}
+
+// The [group] table of one step's sampling scalars and the row -> group map of B batch rows, built as generate()
+// builds them and staged into dyn_dev / grp_dev (stream-ordered).
+static int stage_sample_groups(const vnb_sample_group* groups, int32_t n_groups, int32_t B, DevBuf& dyn_dev,
+                               DevBuf& grp_dev, cudaStream_t st, const char* who) {
+  if (check_groups(groups, n_groups, B, who)) return 1;
+  std::vector<SampleDyn> dyn(n_groups);
+  for (int g = 0; g < n_groups; ++g) dyn[g] = sample_dyn(groups[g]);
+  const std::vector<RowGroup> rowgrp = row_groups(groups, n_groups, B);
+  CK(dyn_dev.alloc(sizeof(SampleDyn) * n_groups));
+  CK(grp_dev.alloc(sizeof(RowGroup) * B));
+  CK(cudaMemcpyAsync(dyn_dev.p, dyn.data(), sizeof(SampleDyn) * n_groups, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+extern "C" {
+
 int32_t vnb_op_gemm(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out, void* out2,
                     const float* bias, int32_t T, int32_t Tpad, void* stream) {
   GemmPlan p;
-  const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
-  if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
-  p.live = g_dbg_live;
+  if (unit_gemm_plan(&p, "vnb_op_gemm", epi, A, W, M, N, K, out, out2, bias, T, Tpad, nullptr, 0, 0.f, 0.f, nullptr,
+                     nullptr))
+    return 1;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -975,106 +1091,40 @@ int32_t vnb_dbg_gemm_ref(const void* A, const void* W, int32_t M, int32_t N, int
   CK(launch_gemm_ref(A, W, M, N, K, out, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
-// The plans below are built exactly as get_workspace() builds the forward's (make_gemm_plan, then the consumer fields
-// or gemm_plan_set_fused_out), so the tests reach every epilogue branch the forward launches.
 int32_t vnb_dbg_gemm_fused(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
                            void* out2, const float* bias, int32_t T, int32_t Tpad, const float* ss_in,
                            int32_t ss_parts, float inv_d, float eps, void* out_bf16, float* ss_out, void* stream) {
   if (epi < VNB_EPI_BF16 || epi > VNB_EPI_BIAS_F32) return fail("vnb_dbg_gemm_fused: epilogue %d not supported", epi);
-  if ((out_bf16 != nullptr || ss_out != nullptr) && epi != VNB_EPI_RESID && epi != VNB_EPI_BIAS_F32)
-    return fail("vnb_dbg_gemm_fused: out_bf16 / ss_out need the RESID or BIAS_F32 epilogue");
-  if ((out_bf16 == nullptr) != (ss_out == nullptr)) return fail("vnb_dbg_gemm_fused: out_bf16 and ss_out go together");
-  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_fused: ss_parts must be >= 1");
   if (epi == VNB_EPI_BIAS_F32 && bias == nullptr) return fail("vnb_dbg_gemm_fused: BIAS_F32 needs a bias");
-  if (epi == VNB_EPI_QKV && (out2 == nullptr || N % 96 != 0 || T < 1 || Tpad < T))
-    return fail("vnb_dbg_gemm_fused: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
   GemmPlan p;
-  const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
-  if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, bias, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
-  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
-  if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
-  p.live = g_dbg_live;
+  if (unit_gemm_plan(&p, "vnb_dbg_gemm_fused", epi, A, W, M, N, K, out, out2, bias, T, Tpad, ss_in, ss_parts, inv_d, eps,
+                     out_bf16, ss_out))
+    return 1;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
-}  // extern "C"
-
-// vnb_dbg_gemm_adapted, and (frames non-null) the adapted QKV of vnb_dbg_gemm_qkv_frames
-static int dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
-                            void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
-                            float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
-                            int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u,
-                            const int32_t* frames, void* stream) {
-  if (epi != VNB_EPI_QKV && epi != VNB_EPI_RESID && epi != VNB_EPI_GEGLU)
-    return fail("vnb_dbg_gemm_adapted: epilogue %d has no adapted variant", epi);
-  if (!adapters || n_adapters < 1 || n_adapters > VNB_MAX_ADAPTERS || !row_adapter || !u || layer < 0)
-    return fail("vnb_dbg_gemm_adapted: need 1..%d adapters, a row map, u and layer >= 0", VNB_MAX_ADAPTERS);
-  if ((out_bf16 != nullptr || ss_out != nullptr) && epi != VNB_EPI_RESID)
-    return fail("vnb_dbg_gemm_adapted: out_bf16 / ss_out need the RESID epilogue");
-  if ((out_bf16 == nullptr) != (ss_out == nullptr)) return fail("vnb_dbg_gemm_adapted: out_bf16 and ss_out go together");
-  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_adapted: ss_parts must be >= 1");
-  if (epi == VNB_EPI_QKV && (out2 == nullptr || N % 96 != 0 || T < 1 || Tpad < T))
-    return fail("vnb_dbg_gemm_adapted: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  std::vector<AdapterDev> tab(VNB_MAX_ADAPTERS);
-  for (int i = 0; i < n_adapters; ++i) {
-    const vnb_adapter_weights& w = adapters[i];
-    const float* ptrs[2 * LORA_SLOTS] = {w.a_qkv, w.b_qkv, w.a_wo, w.b_wo, w.a_w1, w.b_w1, w.a_w2, w.b_w2};
-    for (int s = 0; s < LORA_SLOTS; ++s) { tab[i].a[s] = ptrs[2 * s]; tab[i].b[s] = ptrs[2 * s + 1]; }
-  }
-  std::vector<RowGroup> rowgrp(M);
-  for (int i = 0; i < M; ++i) rowgrp[i] = RowGroup{i, i};  // row m is its own group: grp_adapter = row_adapter
-  GemmPlan p;
-  const int d2 = epi == VNB_EPI_QKV ? (N / 3) * 2 : 0;
-  if (!make_gemm_plan(&p, epi, A, W, M, N, K, out, out2, nullptr, T, Tpad, d2)) return fail("gemm plan: %s", tmap_error());
-  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
-  if (out_bf16 != nullptr) gemm_plan_set_fused_out(&p, out_bf16, ss_out);
-  DevBuf tab_dev, grp_dev;
-  CK(tab_dev.alloc(sizeof(AdapterDev) * VNB_MAX_ADAPTERS));
-  CK(grp_dev.alloc(sizeof(RowGroup) * M));
-  CK(cudaMemcpyAsync(tab_dev.p, tab.data(), sizeof(AdapterDev) * VNB_MAX_ADAPTERS, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * M, cudaMemcpyHostToDevice, st));
-  p.lora.table = tab_dev.as<AdapterDev>();
-  p.lora.grp_adapter = row_adapter;
-  p.lora.rowgrp = grp_dev.as<RowGroup>();
-  p.lora.rows_per_grp = 1;
-  p.lora.slot = epi == VNB_EPI_QKV ? LORA_QKV : epi == VNB_EPI_GEGLU ? LORA_W1 : (K == N ? LORA_WO : LORA_W2);
-  p.lora.layer = layer;
-  p.lora.u = u;
-  p.frames = frames;
-  p.live = g_dbg_live;
-  CK(launch_lora_down(A, M, K, p.lora, p.live, T, st));
-  CK(launch_gemm(p, st));
-  CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
-  return 0;
-}
-
-extern "C" {
 
 int32_t vnb_dbg_gemm_adapted(int32_t epi, const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out,
                              void* out2, int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d,
                              float eps, void* out_bf16, float* ss_out, const vnb_adapter_weights* adapters,
                              int32_t n_adapters, int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
-  return dbg_gemm_adapted(epi, A, W, M, N, K, out, out2, T, Tpad, ss_in, ss_parts, inv_d, eps, out_bf16, ss_out,
-                          adapters, n_adapters, layer, row_adapter, u, nullptr, stream);
+  return dbg_gemm_adapted("vnb_dbg_gemm_adapted", epi, A, W, M, N, K, out, out2, T, Tpad, ss_in, ss_parts, inv_d, eps,
+                          out_bf16, ss_out, adapters, n_adapters, layer, row_adapter, u, nullptr, stream);
 }
 int32_t vnb_dbg_gemm_qkv_frames(const void* A, const void* W, int32_t M, int32_t N, int32_t K, void* out, void* vT,
                                 int32_t T, int32_t Tpad, const float* ss_in, int32_t ss_parts, float inv_d, float eps,
                                 const int32_t* frames, const vnb_adapter_weights* adapters, int32_t n_adapters,
                                 int32_t layer, const int32_t* row_adapter, float* u, void* stream) {
-  if (!frames) return fail("vnb_dbg_gemm_qkv_frames: frames is required");
+  const char* who = "vnb_dbg_gemm_qkv_frames";
+  if (!frames) return fail("%s: frames is required", who);
   if (adapters)
-    return dbg_gemm_adapted(VNB_EPI_QKV, A, W, M, N, K, out, vT, T, Tpad, ss_in, ss_parts, inv_d, eps, nullptr,
+    return dbg_gemm_adapted(who, VNB_EPI_QKV, A, W, M, N, K, out, vT, T, Tpad, ss_in, ss_parts, inv_d, eps, nullptr,
                             nullptr, adapters, n_adapters, layer, row_adapter, u, frames, stream);
-  if (vT == nullptr || N % 96 != 0 || T < 1 || Tpad < T)
-    return fail("vnb_dbg_gemm_qkv_frames: QKV needs vT, N a multiple of 96 and 1 <= T <= Tpad");
-  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_qkv_frames: ss_parts must be >= 1");
   GemmPlan p;
-  if (!make_gemm_plan(&p, VNB_EPI_QKV, A, W, M, N, K, out, vT, nullptr, T, Tpad, (N / 3) * 2))
-    return fail("gemm plan: %s", tmap_error());
-  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
-  p.frames = frames;
-  p.live = g_dbg_live;
+  if (unit_gemm_plan(&p, who, VNB_EPI_QKV, A, W, M, N, K, out, vT, nullptr, T, Tpad, ss_in, ss_parts, inv_d, eps,
+                     nullptr, nullptr))
+    return 1;
+  p.args.frames = frames;
   CK(launch_gemm(p, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
@@ -1083,59 +1133,24 @@ int32_t vnb_dbg_gemm_sample(const void* A, const void* W, const float* bias, int
                             int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token, float temperature,
                             int32_t do_sample, int32_t step, uint32_t seed_lo, uint32_t seed_hi, void* partials,
                             void* stream) {
+  const char* who = "vnb_dbg_gemm_sample";
   if (V % 128 != 0 || V > 1024 || ncc < 0 || C <= ncc || N != (C - ncc) * V || T < 1)
-    return fail("vnb_dbg_gemm_sample: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1");
-  if (!bias || !zcur || !partials) return fail("vnb_dbg_gemm_sample: bias, zcur and partials are required");
-  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_sample: ss_parts must be >= 1");
+    return fail("%s: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1", who);
+  if (!bias || !zcur || !partials) return fail("%s: bias, zcur and partials are required", who);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  SampleDyn d = {};
-  d.inv_temp = inv_temperature(temperature);
-  d.do_sample = do_sample; d.step = step; d.seed_lo = seed_lo; d.seed_hi = seed_hi;
+  vnb_sample_group q = {};
+  q.temperature = temperature; q.do_sample = do_sample; q.step = step; q.seed_lo = seed_lo; q.seed_hi = seed_hi;
   GemmPlan p;
-  if (!make_gemm_plan(&p, VNB_EPI_SAMPLE, A, W, M, N, K, nullptr, nullptr, bias, T, T, 0))
-    return fail("gemm plan: %s", tmap_error());
-  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
-  p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
-  if (stage_sample_dyn(d, st, &p.dyn) || one_group_rows((M + T - 1) / T, &p.rowgrp)) return 1;
-  p.live = g_dbg_live;
+  if (unit_gemm_plan(&p, who, VNB_EPI_SAMPLE, A, W, M, N, K, nullptr, nullptr, bias, T, T, ss_in, ss_parts, inv_d, eps,
+                     nullptr, nullptr))
+    return 1;
+  GemmArgs& a = p.args;
+  a.zcur = zcur; a.partials = reinterpret_cast<float4*>(partials); a.C = C; a.ncc = ncc; a.V = V; a.mask_token = mask_token;
+  if (stage_sample_dyn(sample_dyn(q), st, &a.dyn) || one_group_rows((M + T - 1) / T, &a.rowgrp)) return 1;
   CK(launch_gemm(p, st));
   return 0;
 }
 }  // extern "C"
-
-// The [group] table of one step's sampling scalars and the row -> group map of B batch rows, built as
-// vnb_generate_many builds them and staged into dyn_dev / grp_dev (stream-ordered).
-static int stage_sample_groups(const vnb_sample_group* groups, int32_t n_groups, int32_t B, DevBuf& dyn_dev,
-                               DevBuf& grp_dev, cudaStream_t st, const char* who) {
-  if (n_groups < 1 || n_groups > B) return fail("%s: n_groups %d out of range 1..B (B = %d)", who, n_groups, B);
-  long long total = 0;
-  for (int g = 0; g < n_groups; ++g) {
-    if (groups[g].rows < 1) return fail("%s: group %d has %d rows", who, g, groups[g].rows);
-    total += groups[g].rows;
-  }
-  if (total != B) return fail("%s: group rows sum to %lld, not B = %d", who, total, B);
-  std::vector<SampleDyn> dyn(n_groups);
-  std::vector<RowGroup> rowgrp(B);
-  for (int g = 0, first = 0; g < n_groups; first += groups[g].rows, ++g) {
-    const vnb_sample_group& q = groups[g];
-    SampleDyn& d = dyn[g];
-    d.inv_temp = inv_temperature(q.temperature);
-    d.gamma = q.gamma;
-    d.temp_eff = q.temp_eff;
-    d.do_sample = q.do_sample;
-    d.is_last = q.is_last;
-    d.step = q.step;
-    d.seed_lo = q.seed_lo;
-    d.seed_hi = q.seed_hi;
-    d.top_p = q.top_p;
-    for (int b = first; b < first + q.rows; ++b) rowgrp[b] = RowGroup{g, first};
-  }
-  CK(dyn_dev.alloc(sizeof(SampleDyn) * n_groups));
-  CK(grp_dev.alloc(sizeof(RowGroup) * B));
-  CK(cudaMemcpyAsync(dyn_dev.p, dyn.data(), sizeof(SampleDyn) * n_groups, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(grp_dev.p, rowgrp.data(), sizeof(RowGroup) * B, cudaMemcpyHostToDevice, st));
-  return 0;
-}
 
 // vnb_dbg_sample (paths 0..3) and vnb_dbg_sample_split (path 4: the split combine, the split nucleus draw, the re-mask)
 static int dbg_sample(int32_t path, const float* logits, const void* partials, int32_t* zcur, const int32_t* zorig,
@@ -1187,25 +1202,23 @@ int32_t vnb_dbg_gemm_sample_split(const void* A, const void* W, const float* bia
                                   int32_t T, int32_t C, int32_t ncc, int32_t V, int32_t mask_token,
                                   const vnb_sample_group* groups, int32_t n_groups, void* partials, float* logits,
                                   void* stream) {
+  const char* who = "vnb_dbg_gemm_sample_split";
   if (V % 128 != 0 || V > 1024 || ncc < 0 || C <= ncc || N != (C - ncc) * V || T < 1 || M % T != 0)
-    return fail("vnb_dbg_gemm_sample_split: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1 "
-                "and M a multiple of T");
+    return fail("%s: need V %% 128 == 0, V <= 1024, 0 <= ncc < C, N == (C - ncc) * V, T >= 1 and M a multiple of T", who);
   if (!bias || !zcur || !partials || !logits || !groups)
-    return fail("vnb_dbg_gemm_sample_split: bias, zcur, partials, logits and groups are required");
-  if (ss_in != nullptr && ss_parts < 1) return fail("vnb_dbg_gemm_sample_split: ss_parts must be >= 1");
+    return fail("%s: bias, zcur, partials, logits and groups are required", who);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  DevBuf dyn_dev, grp_dev;
-  if (stage_sample_groups(groups, n_groups, M / T, dyn_dev, grp_dev, st, "vnb_dbg_gemm_sample_split")) return 1;
   GemmPlan p;
-  if (!make_gemm_plan(&p, VNB_EPI_SAMPLE, A, W, M, N, K, nullptr, nullptr, bias, T, T, 0))
-    return fail("gemm plan: %s", tmap_error());
-  p.ss_in = ss_in; p.ss_parts = ss_in ? ss_parts : 0; p.inv_d = inv_d; p.eps = eps;
-  p.zcur = zcur; p.partials = partials; p.C = C; p.ncc = ncc; p.V = V; p.mask_token = mask_token;
-  p.dyn = dyn_dev.as<SampleDyn>();
-  p.rowgrp = grp_dev.as<RowGroup>();
-  p.out = logits;
+  if (unit_gemm_plan(&p, who, VNB_EPI_SAMPLE, A, W, M, N, K, logits, nullptr, bias, T, T, ss_in, ss_parts, inv_d, eps,
+                     nullptr, nullptr))
+    return 1;
+  DevBuf dyn_dev, grp_dev;
+  if (stage_sample_groups(groups, n_groups, M / T, dyn_dev, grp_dev, st, who)) return 1;
+  GemmArgs& a = p.args;
+  a.zcur = zcur; a.partials = reinterpret_cast<float4*>(partials); a.C = C; a.ncc = ncc; a.V = V; a.mask_token = mask_token;
+  a.dyn = dyn_dev.as<SampleDyn>();
+  a.rowgrp = grp_dev.as<RowGroup>();
   p.sample_split = true;
-  p.live = g_dbg_live;
   CK(launch_gemm(p, st));
   CK(cudaStreamSynchronize(st));  // the staged table and row map are freed on return
   return 0;

@@ -48,36 +48,6 @@ constexpr int GEMM_THREADS = 256 + 32;            // two consumer warpgroups + t
 // updated): it gets 8 epilogue warps, two per 32-row quadrant of the tile, splitting the 32-column chunks even / odd.
 template <int EPI> constexpr int gemm_epi_warps() { return (EPI == VNB_EPI_RESID || EPI == VNB_EPI_SAMPLE) ? 8 : 4; }
 
-struct GemmArgs {
-  int M, N, K;
-  int epi;
-  void* out;          // see VNB_EPI_*
-  void* out2;         // vT for EPI_QKV
-  const float* bias;  // EPI_BIAS_F32
-  int T, Tpad;        // EPI_QKV: rows m = b*T + t
-  int d2;             // EPI_QKV: 2*d_model (column where V starts)
-  // ---- fused RMSNorm (reference transformer.py:43-58), see DESIGN.md §4 ----
-  __nv_bfloat16* out_bf16;  // EPI_RESID / EPI_BIAS_F32: bf16 copy of the fp32 output (A operand of the next GEMM)
-  float* ss_out;            // partial row sums of squares of the fp32 output, part p at [p * M + row]: EPI_RESID
-                            // (N/128, M), parts 2j / 2j+1 = even / odd 32-column chunks of n-tile j; EPI_BIAS_F32
-                            // (N/256, M), one part per n-tile
-  const float* ss_in;       // consumers: partial row sums of squares of THEIR A operand; null = no row scaling
-  int ss_parts;             // number of partials to add (fixed order: deterministic)
-  float inv_d, eps;         // row scale = rsqrt(sum * inv_d + eps)
-  // ---- EPI_SAMPLE (see the epilogue) ----
-  const int32_t* zcur;
-  const SampleDyn* dyn;     // this step's row of the (step, group) table
-  const RowGroup* rowgrp;   // (B) group of every batch row
-  float4* partials;
-  int C, ncc, V, mask_token;
-  // ---- adapted variants (ADAPT): per-row LoRA update of the accumulators, see lora_update() ----
-  AdapterRefs lora;
-  const int32_t* frames;    // EPI_QKV: (B) frames of every batch row, null = T; v^T columns t >= frames[b] get 0
-  // ---- launches of calls with different step counts: batch rows >= *live (rows >= *live * T) are idle this iteration;
-  // a tile wholly past them does no work, null = every row is live ----
-  const int32_t* live;
-};
-
 // Rows [0, live_rows) of the launch are live: M without a live bound.
 __device__ __forceinline__ int live_rows(const GemmArgs& g) {
   if (g.live == nullptr) return g.M;
@@ -947,35 +917,27 @@ static cudaError_t launch_epi(const GemmPlan& p, const GemmArgs& g, cudaStream_t
 }
 
 cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st) {
-  GemmArgs g;
-  g.M = p.M; g.N = p.N; g.K = p.K; g.epi = p.epi; g.out = p.out; g.out2 = p.out2; g.bias = p.bias;
-  g.T = p.T; g.Tpad = p.Tpad; g.d2 = p.d2;
-  g.out_bf16 = reinterpret_cast<__nv_bfloat16*>(p.out_bf16); g.ss_out = p.ss_out; g.ss_in = p.ss_in;
-  g.ss_parts = p.ss_parts; g.inv_d = p.inv_d; g.eps = p.eps;
-  g.zcur = p.zcur; g.dyn = p.dyn; g.rowgrp = p.rowgrp; g.partials = reinterpret_cast<float4*>(p.partials);
-  g.C = p.C; g.ncc = p.ncc; g.V = p.V; g.mask_token = p.mask_token;
-  g.lora = p.lora;
-  g.frames = p.epi == VNB_EPI_QKV ? p.frames : nullptr;
-  g.live = p.live;
-  if (p.lora.table != nullptr) {
-    if (!p.lora.grp_adapter || !p.lora.rowgrp || !p.lora.u || p.lora.rows_per_grp < 1) return cudaErrorInvalidValue;
-    switch (p.epi) {
+  GemmArgs g = p.args;
+  if (g.epi != VNB_EPI_QKV) g.frames = nullptr;  // only the QKV epilogue writes per-row padding
+  if (g.lora.table != nullptr) {
+    if (!g.lora.grp_adapter || !g.lora.rowgrp || !g.lora.u || g.lora.rows_per_grp < 1) return cudaErrorInvalidValue;
+    switch (g.epi) {
       case VNB_EPI_QKV: return launch_epi<VNB_EPI_QKV, true>(p, g, st);
       case VNB_EPI_RESID: return launch_epi<VNB_EPI_RESID, true>(p, g, st);
       case VNB_EPI_GEGLU: return launch_epi<VNB_EPI_GEGLU, true>(p, g, st);
       default: return cudaErrorInvalidValue;  // the embedding and the classifier carry no LoRA
     }
   }
-  switch (p.epi) {
+  switch (g.epi) {
     case VNB_EPI_BF16: return launch_epi<VNB_EPI_BF16>(p, g, st);
     case VNB_EPI_QKV: return launch_epi<VNB_EPI_QKV>(p, g, st);
     case VNB_EPI_RESID: return launch_epi<VNB_EPI_RESID>(p, g, st);
     case VNB_EPI_GEGLU: return launch_epi<VNB_EPI_GEGLU>(p, g, st);
     case VNB_EPI_BIAS_F32: return launch_epi<VNB_EPI_BIAS_F32>(p, g, st);
     case VNB_EPI_SAMPLE:
-      if (!p.zcur || !p.dyn || !p.rowgrp || !p.partials || !p.bias || p.V % 128 != 0 || p.V > 1024) return cudaErrorInvalidValue;
+      if (!g.zcur || !g.dyn || !g.rowgrp || !g.partials || !g.bias || g.V % 128 != 0 || g.V > 1024) return cudaErrorInvalidValue;
       if (p.sample_split) {
-        if (!p.out) return cudaErrorInvalidValue;
+        if (!g.out) return cudaErrorInvalidValue;
         return launch_epi<VNB_EPI_SAMPLE, false, true>(p, g, st);
       }
       return launch_epi<VNB_EPI_SAMPLE>(p, g, st);

@@ -1,6 +1,7 @@
 // vampnet_b200 — internal launcher declarations shared by the .cu translation units.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -73,42 +74,45 @@ cudaError_t launch_lora_down(const void* y, int M, int K, const AdapterRefs& r, 
                              cudaStream_t st);
 
 // ---- GEMM ----
-struct GemmPlan {
-  CUtensorMap tmA, tmB;
-  CUtensorMap tmBh;  // W with a 128-row box: the half tile each CTA of a pair fetches and multicasts (gemm_wgmma.cu, PAIR)
-  int M = 0, N = 0, K = 0, epi = 0;
-  void* out = nullptr;
-  void* out2 = nullptr;
-  const float* bias = nullptr;
-  int T = 1, Tpad = 1, d2 = 0;
-  // fused RMSNorm plumbing (see GemmArgs in gemm_wgmma.cu)
-  void* out_bf16 = nullptr;
-  float* ss_out = nullptr;
-  const float* ss_in = nullptr;
-  int ss_parts = 0;
-  float inv_d = 0.f, eps = 0.f;
-  // VNB_EPI_SAMPLE (the classifier of the generate loop): the logits are sampled in the epilogue instead of being stored
-  const int32_t* zcur = nullptr;     // (B, T, C) current tokens: only still-masked positions are sampled
-  const SampleDyn* dyn = nullptr;    // this step's scalars, one per group (device memory: graph replay safe)
-  const RowGroup* rowgrp = nullptr;  // (B) group of every batch row
-  void* partials = nullptr;          // (M * Cp * V/128) float4 records, see sample_combine_kernel
-  // a launch of nucleus (top-p) and plain groups: the rows of nucleus groups store their logits to `out` (the
-  // materialising epilogue's layout, still-masked positions only) and leave no records
-  bool sample_split = false;
-  int C = 0, ncc = 0, V = 0, mask_token = 0;
-  // adapted variant of QKV / RESID / GEGLU (null table: the plain kernel): acc += u[row] . B'[col] for adapted rows
+// The arguments every GEMM kernel takes by value (gemm_wgmma.cu).
+struct GemmArgs {
+  int M, N, K;
+  int epi;
+  void* out;          // see VNB_EPI_*
+  void* out2;         // vT for EPI_QKV
+  const float* bias;  // EPI_BIAS_F32
+  int T, Tpad;        // EPI_QKV: rows m = b*T + t
+  int d2;             // EPI_QKV: 2*d_model (column where V starts)
+  // ---- fused RMSNorm (reference transformer.py:43-58), see DESIGN.md §4 ----
+  __nv_bfloat16* out_bf16;  // EPI_RESID / EPI_BIAS_F32: bf16 copy of the fp32 output (A operand of the next GEMM)
+  float* ss_out;            // partial row sums of squares of the fp32 output, part p at [p * M + row]: EPI_RESID
+                            // (N/128, M), parts 2j / 2j+1 = even / odd 32-column chunks of n-tile j; EPI_BIAS_F32
+                            // (N/256, M), one part per n-tile
+  const float* ss_in;       // consumers: partial row sums of squares of THEIR A operand; null = no row scaling
+  int ss_parts;             // number of partials to add (fixed order: deterministic)
+  float inv_d, eps;         // row scale = rsqrt(sum * inv_d + eps)
+  // ---- EPI_SAMPLE (the classifier of the generate loop): the logits are sampled in the epilogue, not stored ----
+  const int32_t* zcur;      // (B, T, C) current tokens: only still-masked positions are sampled
+  const SampleDyn* dyn;     // this step's row of the (step, group) table (device memory: graph replay safe)
+  const RowGroup* rowgrp;   // (B) group of every batch row
+  float4* partials;         // (M * Cp * V/128) records, see sample_combine_kernel
+  int C, ncc, V, mask_token;
+  // ---- adapted variants of QKV / RESID / GEGLU (null table: the plain kernel): acc += u[row] . B'[col] for adapted
+  // rows, see lora_update() ----
   AdapterRefs lora;
-  // VNB_EPI_QKV of a launch whose calls have different lengths: (B) frames of every batch row; v^T column t of batch row
-  // b is written as 0 for t >= frames[b] (null: every row has T frames)
-  const int32_t* frames = nullptr;
-  // launches of calls with different step counts: (1) the number of live batch rows this iteration (device); tiles
-  // wholly at or past row live[0] * T exit at once (null: every row is live)
-  const int32_t* live = nullptr;
+  const int32_t* frames;    // EPI_QKV: (B) frames of every batch row, null = T; v^T columns t >= frames[b] get 0
+  // ---- launches of calls with different step counts: batch rows >= *live (rows >= *live * T) are idle this iteration;
+  // a tile wholly past them does no work, null = every row is live ----
+  const int32_t* live;
 };
-// Fills the tensor maps; A (M,K) bf16, W (N,K) bf16.
-bool make_gemm_plan(GemmPlan* p, int epi, const void* A, const void* W, int M, int N, int K, void* out, void* out2,
-                    const float* bias, int T, int Tpad, int d2);
-bool gemm_plan_set_fused_out(GemmPlan* p, void* out_bf16, float* ss_out);
+struct GemmPlan {
+  CUtensorMap tmA, tmB;  // A (M,K) bf16, W (N,K) bf16
+  CUtensorMap tmBh;  // W with a 128-row box: the half tile each CTA of a pair fetches and multicasts (gemm_wgmma.cu, PAIR)
+  // EPI_SAMPLE in a launch of nucleus (top-p) and plain groups: the rows of nucleus groups store their logits to `out`
+  // (the materialising epilogue's layout, still-masked positions only) and leave no records
+  bool sample_split = false;
+  GemmArgs args{};
+};
 cudaError_t launch_gemm(const GemmPlan& p, cudaStream_t st);
 cudaError_t prepare_gemm();  // per-device kernel attributes; call outside stream capture
 void set_gemm_pair(int on);  // 1: CTA pairs (clusters of two sharing the W tile), 0: single-CTA tiles
