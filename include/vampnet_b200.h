@@ -499,12 +499,24 @@ int32_t vnb_dbg_beat_from_envelope(const float* envelope, int32_t B, int32_t F, 
  * vnb_pitch_workspace_bytes(...) bytes (about 0.6 GB per 10 s row at 44.1 kHz and +12 semitones).  The float64 DFT
  * bases are built on the host on the first call for a (device, n_fft) and cached; that first call allocates and
  * uploads them.  Refused: a NULL buffer, a workspace that is too small, rows outside 1..65535, n_fft outside 16..4096,
- * hop < 1 or hop > n_fft, N <= n_fft / 2, sample_rate or new_freq < 1, rate <= 0 or not finite. */
+ * hop < 1 or hop > n_fft, N <= n_fft / 2, sample_rate or new_freq < 1, rate <= 0 or not finite, and an empty istft
+ * signal (even n_fft with one stretched frame, ceil(F / rate) = 1, as torch.istft refuses it). */
 int32_t vnb_pitch_workspace_bytes(int32_t rows, int32_t N, int32_t sample_rate, int32_t new_freq, int32_t n_fft,
                                   int32_t hop, double rate, uint64_t* bytes);
 int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t sample_rate, int32_t new_freq,
                         int32_t n_fft, int32_t hop, double rate, void* workspace, uint64_t workspace_bytes, float* out,
                         void* stream);
+/* Test-only: where vnb_pitch_shift with the same arguments keeps its float64 intermediates in the workspace, as
+ * byte offsets (-1: not kept for these arguments), and the shapes it derives:
+ *   offsets[0] spectrum (rows, F, nb) complex: X as the forward DFT wrote it when rate == 1; (|X|, angle X) when
+ *              rate != 1
+ *   offsets[1] stretched spectrum (rows, F2, nb) complex, after the vocoder (-1 when rate == 1)
+ *   offsets[2] inverse-DFT frames (rows, F2, n_fft)
+ *   offsets[3] overlap-added signal (rows, L)
+ * with nb = n_fft / 2 + 1 and dims = {F, F2, L, target}.  Same refusals as vnb_pitch_workspace_bytes, and NULL
+ * offsets or dims. */
+int32_t vnb_dbg_pitch_layout(int32_t rows, int32_t N, int32_t sample_rate, int32_t new_freq, int32_t n_fft,
+                             int32_t hop, double rate, int64_t* offsets, int64_t* dims);
 /* test hook: the phase vocoder's time steps, out[i] = float(rate) * float(i) for i < n, fp32 DEVICE */
 int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* stream);
 /* ---- validation metrics (the reference's scripts/exp/train.py val_loop / _metrics / accuracy, train.py:155-213,

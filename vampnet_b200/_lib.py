@@ -154,6 +154,7 @@ _SIGS = {
     "vnb_pitch_workspace_bytes": (C.c_int32, [C.c_int32] * 6 + [C.c_double, C.POINTER(C.c_uint64)]),
     "vnb_pitch_shift": (C.c_int32, [C.c_void_p] + [C.c_int32] * 6 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,
                                                                       C.c_void_p]),
+    "vnb_dbg_pitch_layout": (C.c_int32, [C.c_int32] * 6 + [C.c_double, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "vnb_dbg_pitch_time_steps": (C.c_int32, [C.c_double, C.c_int32, C.c_void_p, C.c_void_p]),
     "vnb_xent_metrics_workspace_bytes": (C.c_int32, [C.c_int32, C.c_int64, C.POINTER(C.c_uint64)]),
     "vnb_xent_metrics": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32] * 5 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,

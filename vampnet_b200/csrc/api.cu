@@ -1318,8 +1318,12 @@ static int32_t pitch_args(const char* fn, int32_t rows, int32_t N, int32_t sr, i
   if (N <= n_fft / 2) return fail("%s: need N > n_fft // 2 for the reflect padding (got N = %d, n_fft = %d)", fn, N, n_fft);
   if (sr < 1 || new_freq < 1) return fail("%s: need sample_rate >= 1 and new_freq >= 1 (got %d, %d)", fn, sr, new_freq);
   if (!(rate > 0) || !std::isfinite(rate)) return fail("%s: need a finite rate > 0 (got %g)", fn, rate);
-  if (pitch_plan(rows, N, sr, new_freq, n_fft, hop, rate, p))
+  const int rc = pitch_plan(rows, N, sr, new_freq, n_fft, hop, rate, p);
+  if (rc == 1)
     return fail("%s: ceil(F / rate) stretched frames is out of range (N = %d, hop = %d, rate = %g)", fn, N, hop, rate);
+  if (rc)
+    return fail("%s: one stretched frame of even n_fft = %d leaves an empty istft signal (N = %d, hop = %d, rate = %g)",
+                fn, n_fft, N, hop, rate);
   return 0;
 }
 int32_t vnb_pitch_workspace_bytes(int32_t rows, int32_t N, int32_t sr, int32_t new_freq, int32_t n_fft, int32_t hop,
@@ -1342,6 +1346,19 @@ int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t s
   const double *fwd = nullptr, *inv = nullptr;
   CK(pitch_basis(n_fft, &fwd, &inv));
   CK(launch_pitch_shift(samples, p, fwd, inv, workspace, out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_pitch_layout(int32_t rows, int32_t N, int32_t sr, int32_t new_freq, int32_t n_fft, int32_t hop,
+                             double rate, int64_t* offsets, int64_t* dims) {
+  if (!offsets || !dims) return fail("vnb_dbg_pitch_layout: offsets and dims are required");
+  PitchPlan p;
+  if (int32_t rc = pitch_args("vnb_dbg_pitch_layout", rows, N, sr, new_freq, n_fft, hop, rate, &p)) return rc;
+  const PitchLayout l = pitch_layout(p);
+  offsets[0] = (int64_t)l.spec;
+  offsets[1] = p.stretch ? (int64_t)l.stretched : -1;
+  offsets[2] = (int64_t)l.frames;
+  offsets[3] = (int64_t)l.y;
+  dims[0] = p.F; dims[1] = p.F2; dims[2] = p.L; dims[3] = p.target;
   return 0;
 }
 int32_t vnb_dbg_pitch_time_steps(double rate, int32_t n, float* out, void* stream) {

@@ -244,8 +244,14 @@ struct PitchPlan {
   long long L = 0, target = 0, orig_g = 1, new_g = 1;
   bool stretch = false, resample = false;
 };
-// 0, or 1 when the stretched frame count is out of range
+// 0; 1 when the stretched frame count is out of range, 2 when the istft length L is 0 (even n_fft, F2 = 1)
 int pitch_plan(int rows, int N, int sr, int new_freq, int n_fft, int hop, double rate, PitchPlan* p);
+// the workspace of one call, as byte offsets: spectrum (then (|X|, angle) in place), the stretched spectrum and the
+// vocoder's chunk sums (rate != 1 only; stretched == spec otherwise), the inverse-DFT frames, the overlap-added signal
+struct PitchLayout {
+  size_t spec = 0, stretched = 0, chunk = 0, frames = 0, y = 0, total = 0;
+};
+PitchLayout pitch_layout(const PitchPlan& p);
 size_t pitch_workspace_bytes(const PitchPlan& p);
 // float64 forward (n_fft x 2 n_bins) and inverse (2 n_bins x n_fft) DFT bases, zero padded to the GEMM tiles; built on
 // the host once per (device, n_fft), then cached

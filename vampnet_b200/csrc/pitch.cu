@@ -297,6 +297,7 @@ int pitch_plan(int rows, int N, int sr, int new_freq, int n_fft, int hop, double
   q.F2 = (int)F2;
   q.nchunks = (q.F2 + CH - 1) / CH;
   q.L = (long long)n_fft - 2LL * (n_fft / 2) + (long long)hop * (q.F2 - 1);  // torch.istft, center=True, length=None
+  if (q.L < 1) return 2;  // one stretched frame of even n_fft: torch.istft refuses the empty signal
   q.resample = new_freq != sr;
   if (q.resample) {
     const long long g = std::gcd((long long)sr, (long long)new_freq);
@@ -314,15 +315,21 @@ int pitch_plan(int rows, int N, int sr, int new_freq, int n_fft, int hop, double
   return 0;
 }
 
-size_t pitch_workspace_bytes(const PitchPlan& p) {
+PitchLayout pitch_layout(const PitchPlan& p) {
   const size_t R = (size_t)p.rows, z = sizeof(double);
-  size_t b = align256(R * p.F * p.nb * 2 * z);                      // spectrum, then (|X|, angle)
-  if (p.stretch) b += align256(R * p.F2 * p.nb * 2 * z);            // stretched spectrum
-  if (p.stretch) b += align256(R * p.nchunks * p.nb * z);           // chunk sums
-  b += align256(R * p.F2 * p.n_fft * z);                            // inverse DFT frames
-  b += align256(R * p.L * z);                                       // overlap-added signal
-  return b;
+  PitchLayout l;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += align256(bytes); return at; };
+  l.spec = take(R * p.F * p.nb * 2 * z);                            // spectrum, then (|X|, angle)
+  l.stretched = p.stretch ? take(R * p.F2 * p.nb * 2 * z) : l.spec;  // stretched spectrum
+  l.chunk = p.stretch ? take(R * p.nchunks * p.nb * z) : 0;          // chunk sums
+  l.frames = take(R * p.F2 * p.n_fft * z);                          // inverse DFT frames
+  l.y = take(R * p.L * z);                                          // overlap-added signal
+  l.total = o;
+  return l;
 }
+
+size_t pitch_workspace_bytes(const PitchPlan& p) { return pitch_layout(p).total; }
 
 cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv) {
   int dev = 0;
@@ -364,21 +371,13 @@ cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv) {
 
 cudaError_t launch_pitch_shift(const float* x, const PitchPlan& p, const double* fwd, const double* inv, void* ws,
                                float* out, cudaStream_t st) {
-  const size_t R = (size_t)p.rows, z = sizeof(double);
   char* w = reinterpret_cast<char*>(ws);
-  double* spec = reinterpret_cast<double*>(w);
-  w += align256(R * p.F * p.nb * 2 * z);
-  double* stretched = spec;
-  double* chunk = nullptr;
-  if (p.stretch) {
-    stretched = reinterpret_cast<double*>(w);
-    w += align256(R * p.F2 * p.nb * 2 * z);
-    chunk = reinterpret_cast<double*>(w);
-    w += align256(R * p.nchunks * p.nb * z);
-  }
-  double* frames = reinterpret_cast<double*>(w);
-  w += align256(R * p.F2 * p.n_fft * z);
-  double* y = reinterpret_cast<double*>(w);
+  const PitchLayout l = pitch_layout(p);
+  double* spec = reinterpret_cast<double*>(w + l.spec);
+  double* stretched = reinterpret_cast<double*>(w + l.stretched);
+  double* chunk = p.stretch ? reinterpret_cast<double*>(w + l.chunk) : nullptr;
+  double* frames = reinterpret_cast<double*>(w + l.frames);
+  double* y = reinterpret_cast<double*>(w + l.y);
 
   const int nb = p.nb;
   GemmA fa{};
@@ -387,7 +386,7 @@ cudaError_t launch_pitch_shift(const float* x, const PitchPlan& p, const double*
       fa, fwd, round_up(p.n_fft, BK), round_up(2 * nb, BN), spec, 2 * nb, 2 * nb);
   count_launch();
   if (p.stretch) {
-    const long long n = (long long)R * p.F * nb;
+    const long long n = (long long)p.rows * p.F * nb;
     to_polar_kernel<<<grid_for(n, 256), 256, 0, st>>>(reinterpret_cast<double2*>(spec), n);
     count_launch();
     VocoderArgs va;
