@@ -551,6 +551,36 @@ int32_t vnb_xent_metrics(const float* logits, const int64_t* z, const int64_t* m
 /* test hook: the per-row records (B * S vnb_xent_row, DEVICE) of vnb_xent_metrics; same refusals */
 int32_t vnb_dbg_xent_rows(const float* logits, const int64_t* z, int32_t B, int32_t C, int32_t T, int32_t ncc,
                           int32_t V, vnb_xent_row* rows, void* stream);
+/* ---- mel spectrogram and multi-scale mel distance (audiotools' AudioSignal.mel_spectrogram and
+ *      metrics.spectral.MelSpectrogramLoss, restated on the device; DESIGN.md §13).  Nothing here synchronises. -----
+ * One scale: |torch.stft(x, n_fft, hop, window=periodic Hann, center=True, pad_mode="reflect")| in fp32, F = 1 + N / hop
+ * frames, projected on librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax) (Slaney scale and norm, float32 weights).
+ * fmax is given explicitly (audiotools' None is sr / 2). */
+typedef struct vnb_mel_scale {
+  int32_t n_fft, hop, n_mels;
+  double fmin, fmax;
+} vnb_mel_scale;
+/* samples (rows, N) fp32 DEVICE -> out (rows, n_mels, F) fp32 DEVICE.  A row's output depends on that row only, so it
+ * equals the row run alone, bit for bit.  The window, twiddles and filterbank are built on the host in float64 on the
+ * first call for a (device, sr, n_fft, n_mels, fmin, fmax) and cached; that first call allocates and uploads them.
+ * Refused: a NULL buffer, rows outside 1..65535, sr < 1, n_fft not a power of two in 32..4096, N <= n_fft / 2 (the
+ * reflect padding), hop < 1, n_mels outside 1..4096, fmin < 0, fmax <= fmin. */
+int32_t vnb_mel_spectrogram(const float* samples, int32_t rows, int32_t N, int32_t sr, const vnb_mel_scale* scale,
+                            float* out, void* stream);
+/* x and y (B, C, N) fp32 DEVICE, the same sample rate.  For each scale, with X and Y the (B, C, n_mels, F) spectrograms:
+ *   loss += log_weight * mean|log10(max(X, clamp_eps)^pow) - log10(max(Y, clamp_eps)^pow)| + mag_weight * mean|X - Y|
+ * over all B C n_mels F elements (item_loss[b]: over item b's C n_mels F), clamp, pow (as pow * log10) and log10 in
+ * float64, every sum in float64 in a fixed order, each result rounded to fp32 once.  loss (1) fp32 DEVICE; item_loss
+ * (B) fp32 DEVICE or NULL.  An item's loss depends on that item only, so it equals the item run alone, bit for bit.
+ * workspace: DEVICE, at least vnb_mel_workspace_bytes(B, C, N, scales, n_scales) bytes.  Refused: a NULL buffer,
+ * B * C outside 1..65535, n_scales outside 1..16, any scale refused as by vnb_mel_spectrogram, clamp_eps <= 0 or not
+ * finite, pow, log_weight or mag_weight not finite, a workspace that is too small. */
+int32_t vnb_mel_workspace_bytes(int32_t B, int32_t C, int32_t N, int32_t sr, const vnb_mel_scale* scales,
+                                int32_t n_scales, uint64_t* bytes);
+int32_t vnb_mel_loss(const float* x, const float* y, int32_t B, int32_t C, int32_t N, int32_t sr,
+                     const vnb_mel_scale* scales, int32_t n_scales, double clamp_eps, double pow, double log_weight,
+                     double mag_weight, void* workspace, uint64_t workspace_bytes, float* loss, float* item_loss,
+                     void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

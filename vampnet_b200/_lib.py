@@ -59,6 +59,11 @@ class SampleGroup(C.Structure):
     ]
 
 
+class MelScale(C.Structure):
+    _fields_ = [("n_fft", C.c_int32), ("hop", C.c_int32), ("n_mels", C.c_int32), ("fmin", C.c_double),
+                ("fmax", C.c_double)]
+
+
 _SIGS = {
     "vnb_abi_version": (C.c_int32, []),
     "vnb_last_error": (C.c_char_p, []),
@@ -160,6 +165,10 @@ _SIGS = {
     "vnb_xent_metrics": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32] * 5 + [C.c_double, C.c_void_p, C.c_uint64, C.c_void_p,
                                                                           C.c_void_p, C.c_void_p]),
     "vnb_dbg_xent_rows": (C.c_int32, [C.c_void_p] * 2 + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p]),
+    "vnb_mel_spectrogram": (C.c_int32, [C.c_void_p] + [C.c_int32] * 3 + [C.POINTER(MelScale), C.c_void_p, C.c_void_p]),
+    "vnb_mel_workspace_bytes": (C.c_int32, [C.c_int32] * 4 + [C.POINTER(MelScale), C.c_int32, C.POINTER(C.c_uint64)]),
+    "vnb_mel_loss": (C.c_int32, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.POINTER(MelScale), C.c_int32] + [C.c_double] * 4
+                     + [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
     "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,

@@ -103,6 +103,19 @@ class AudioSignal:
             self.audio_data = self.audio_data[..., before:-after]
         return self
 
+    def truncate_samples(self, length_in_samples: int):
+        """Keep the first `length_in_samples` samples, in place (audiotools' truncate_samples)."""
+        self.audio_data = self.audio_data[..., :int(length_in_samples)]
+        return self
+
+    def mel_spectrogram(self, n_mels: int = 80, mel_fmin: float = 0.0, mel_fmax: float = None,
+                        window_length: int = None, hop_length: int = None, window_type: str = None):
+        """(batch, channels, n_mels, frames) fp32 magnitude mel spectrogram, audiotools' definition, computed on the
+        GPU (vampnet_b200.metrics.mel_spectrogram, DESIGN.md §13)."""
+        from .metrics import mel_spectrogram
+        return mel_spectrogram(self.audio_data, self.sample_rate, n_mels, mel_fmin, mel_fmax, window_length,
+                               hop_length, window_type)
+
     def resample(self, sample_rate: int):
         """Band-limited (Kaiser-windowed sinc) polyphase resampling as one strided conv."""
         sample_rate = int(sample_rate)

@@ -1406,4 +1406,61 @@ int32_t vnb_dbg_xent_rows(const float* logits, const int64_t* z, int32_t B, int3
   return 0;
 }
 
+// ---- mel spectrogram and multi-scale mel distance (mel.cu) ----
+static int32_t mel_scale_args(const char* fn, int32_t N, int32_t sr, const vnb_mel_scale& s) {
+  if (sr < 1) return fail("%s: need sr >= 1 (got %d)", fn, sr);
+  if (s.n_fft < MEL_MIN_NFFT || s.n_fft > MEL_MAX_NFFT || (s.n_fft & (s.n_fft - 1)))
+    return fail("%s: n_fft = %d; a power of two in %d..%d is supported", fn, s.n_fft, MEL_MIN_NFFT, MEL_MAX_NFFT);
+  if (N <= s.n_fft / 2)
+    return fail("%s: need N > n_fft // 2 for the reflect padding (got N = %d, n_fft = %d)", fn, N, s.n_fft);
+  if (s.hop < 1) return fail("%s: need hop >= 1 (got %d)", fn, s.hop);
+  if (s.n_mels < 1 || s.n_mels > MEL_MAX_MELS) return fail("%s: n_mels = %d; 1..%d are supported", fn, s.n_mels, MEL_MAX_MELS);
+  if (!(s.fmin >= 0.0) || !(s.fmax > s.fmin) || !std::isfinite(s.fmax))
+    return fail("%s: need 0 <= fmin < fmax, both finite (got fmin = %g, fmax = %g)", fn, s.fmin, s.fmax);
+  return 0;
+}
+int32_t vnb_mel_spectrogram(const float* samples, int32_t rows, int32_t N, int32_t sr, const vnb_mel_scale* scale,
+                            float* out, void* stream) {
+  if (!samples || !scale || !out) return fail("vnb_mel_spectrogram: samples, scale and out are required");
+  if (rows < 1 || rows > 65535) return fail("vnb_mel_spectrogram: need 1 <= rows <= 65535 (got %d)", rows);
+  if (int32_t rc = mel_scale_args("vnb_mel_spectrogram", N, sr, *scale)) return rc;
+  CK(launch_mel_spectrogram(samples, rows, N, sr, *scale, out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+static int32_t mel_loss_args(const char* fn, int32_t B, int32_t C, int32_t N, int32_t sr, const vnb_mel_scale* scales,
+                             int32_t n_scales) {
+  if (B < 1 || C < 1 || (int64_t)B * C > 65535)
+    return fail("%s: need B, C >= 1 and B * C <= 65535 (got B = %d, C = %d)", fn, B, C);
+  if (!scales) return fail("%s: scales is NULL", fn);
+  if (n_scales < 1 || n_scales > MEL_MAX_SCALES) return fail("%s: n_scales = %d; 1..%d are supported", fn, n_scales, MEL_MAX_SCALES);
+  for (int i = 0; i < n_scales; ++i)
+    if (int32_t rc = mel_scale_args(fn, N, sr, scales[i])) return rc;
+  return 0;
+}
+int32_t vnb_mel_workspace_bytes(int32_t B, int32_t C, int32_t N, int32_t sr, const vnb_mel_scale* scales,
+                                int32_t n_scales, uint64_t* bytes) {
+  if (!bytes) return fail("vnb_mel_workspace_bytes: bytes is NULL");
+  if (int32_t rc = mel_loss_args("vnb_mel_workspace_bytes", B, C, N, sr, scales, n_scales)) return rc;
+  *bytes = mel_loss_plan(B, C, N, sr, scales, n_scales).total;
+  return 0;
+}
+int32_t vnb_mel_loss(const float* x, const float* y, int32_t B, int32_t C, int32_t N, int32_t sr,
+                     const vnb_mel_scale* scales, int32_t n_scales, double clamp_eps, double pow, double log_weight,
+                     double mag_weight, void* workspace, uint64_t workspace_bytes, float* loss, float* item_loss,
+                     void* stream) {
+  if (!x || !y || !workspace || !loss) return fail("vnb_mel_loss: x, y, workspace and loss are required");
+  if (int32_t rc = mel_loss_args("vnb_mel_loss", B, C, N, sr, scales, n_scales)) return rc;
+  if (!(clamp_eps > 0.0) || !std::isfinite(clamp_eps))
+    return fail("vnb_mel_loss: need a finite clamp_eps > 0 (got %g)", clamp_eps);
+  if (!std::isfinite(pow) || !std::isfinite(log_weight) || !std::isfinite(mag_weight))
+    return fail("vnb_mel_loss: pow, log_weight and mag_weight must be finite");
+  const MelLossPlan p = mel_loss_plan(B, C, N, sr, scales, n_scales);
+  if (workspace_bytes < p.total)
+    return fail("vnb_mel_loss: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
+                (unsigned long long)p.total);
+  CK(launch_mel_loss(x, y, p, clamp_eps, pow, log_weight, mag_weight, workspace, loss, item_loss,
+                     reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 }  // extern "C"

@@ -184,6 +184,20 @@ cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cud
 // groups from `partials`, the nucleus draw the rows of top-p groups from a.logits, then the re-mask
 cudaError_t launch_sample_split_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
 
+// ---- host tables shared by onset.cu and mel.cu: built in float64, rounded to fp32 once, then cached (onset.cu) ----
+struct FftTables {
+  const float2* twiddle;  // (n_fft / 2 + 1) exp(-2 pi i k / n_fft), for fft.cuh
+  const float* window;    // (n_fft) periodic Hann
+};
+cudaError_t fft_tables(int n_fft, FftTables* out);  // per (device, n_fft)
+// librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm="slaney", dtype=float32), nonzero ranges only
+struct MelBank {
+  const float* w;       // band m's weights at [off[m], off[m + 1]), for bins lo[m], lo[m] + 1, ...
+  const int32_t* off;   // (n_mels + 1)
+  const int32_t* lo;    // (n_mels) first nonzero bin of band m (0 for an empty band)
+};
+cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out);  // per (device, all)
+
 // ---- onset detection (onset.cu; librosa 0.10 onset_detect restated, DESIGN.md §9) ----
 // peak_pick windows of onset_detect's defaults at (sr, hop), and the envelope's left padding lag + n_fft // (2 hop)
 struct OnsetGeometry {
@@ -273,5 +287,28 @@ cudaError_t launch_xent_rows(const float* logits, const int64_t* z, int B, int C
 cudaError_t launch_xent_metrics(const float* logits, const int64_t* z, const int64_t* mask, const double* r, int B,
                                 int C, int T, int ncc, int V, double eps, void* workspace, float* out,
                                 int32_t* ambiguous, cudaStream_t st);
+
+// ---- mel spectrogram and multi-scale mel distance (mel.cu; audiotools' MelSpectrogramLoss restated, DESIGN.md §13) ----
+constexpr int MEL_MIN_NFFT = 32, MEL_MAX_NFFT = 4096, MEL_MAX_MELS = 4096, MEL_MAX_SCALES = 16;
+struct MelScalePlan {
+  int n_fft = 0, hop = 0, n_mels = 0, F = 0;  // F = 1 + N / hop frames
+  double fmin = 0.0, fmax = 0.0;
+  long long elems = 0;  // C * n_mels * F: one item's spectrogram
+  int chunks = 0;       // reduction CTAs per item
+  size_t partial = 0;   // first of this scale's (B, chunks) partial sums in the workspace's partial array
+};
+struct MelLossPlan {
+  int B = 0, C = 0, N = 0, sr = 0, n_scales = 0;
+  MelScalePlan s[MEL_MAX_SCALES];
+  size_t x_spec = 0, y_spec = 0, partials = 0, items = 0, total = 0;  // workspace byte offsets and size
+};
+MelLossPlan mel_loss_plan(int B, int C, int N, int sr, const vnb_mel_scale* scales, int n_scales);
+// samples (rows, N) fp32 -> out (rows, n_mels, F) fp32 |STFT| projected on the Slaney filterbank
+cudaError_t launch_mel_spectrogram(const float* samples, int rows, int N, int sr, const vnb_mel_scale& s, float* out,
+                                   cudaStream_t st);
+// loss (1) and, when not null, item_loss (B): fp32, formed in float64 and rounded once
+cudaError_t launch_mel_loss(const float* x, const float* y, const MelLossPlan& p, double clamp_eps, double pow,
+                            double log_weight, double mag_weight, void* workspace, float* loss, float* item_loss,
+                            cudaStream_t st);
 
 }  // namespace vnb

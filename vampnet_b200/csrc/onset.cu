@@ -8,25 +8,25 @@
 //                       minimum tests in parallel, then one warp walks them 32 frames at a time for peak_pick's
 //                       wait rule and onset_backtrack
 //   onset_mask_kernel   the reference's mask[:, :, idx - w:idx + w] = 0 loop, with Python slice semantics
-// DESIGN.md §9 has the numerics; oracle/onset_oracle.py restates the algorithm in float64.
+// DESIGN.md §9 has the numerics; oracle/onset_oracle.py restates the algorithm in float64.  The FFT (fft.cuh) and
+// the host tables built here (fft_tables, mel_filterbank) are shared with mel.cu.
 #include <algorithm>
+#include <initializer_list>
 #include <cmath>
 #include <cstring>
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <utility>
 #include <vector>
 
+#include "fft.cuh"
 #include "kernels.h"
 
 namespace vnb {
 
 namespace {
 constexpr int NFFT = 2048, NH = NFFT / 2, NBINS = NH + 1, NMELS = 128, THREADS = 256;
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
-}
 
 __global__ void __launch_bounds__(THREADS) onset_spec_kernel(const float* __restrict__ samples, int N, int F, int hop,
                                                              OnsetTables t, float* __restrict__ db) {
@@ -42,26 +42,10 @@ __global__ void __launch_bounds__(THREADS) onset_spec_kernel(const float* __rest
     z[__brev(m) >> 22] = make_float2(a * t.window[2 * m], c * t.window[2 * m + 1]);  // bit-reversed 10-bit index
   }
   __syncthreads();
-  // radix-2 decimation in time; stage `len` uses W_len^k = twiddle[k * NFFT / len]
-  for (int len = 2; len <= NH; len <<= 1) {
-    const int half = len >> 1, step = NFFT / len;
-    for (int j = threadIdx.x; j < NH / 2; j += THREADS) {
-      const int k = j & (half - 1);
-      const int i0 = (j - k) * 2 + k, i1 = i0 + half;
-      const float2 u = z[i0], v = cmul(z[i1], t.twiddle[k * step]);
-      z[i0] = make_float2(u.x + v.x, u.y + v.y);
-      z[i1] = make_float2(u.x - v.x, u.y - v.y);
-    }
-    __syncthreads();
-  }
-  // real split: E = (Z[k] + conj Z[NH-k]) / 2, O = (Z[k] - conj Z[NH-k]) / 2i, X[k] = E + W_NFFT^k O
+  fft_radix2<NFFT>(z, t.twiddle, threadIdx.x, THREADS);
   for (int k = threadIdx.x; k < NBINS; k += THREADS) {
-    const float2 zk = z[k & (NH - 1)], zn = z[(NH - k) & (NH - 1)];
-    const float2 e = make_float2(0.5f * (zk.x + zn.x), 0.5f * (zk.y - zn.y));
-    const float2 o = make_float2(0.5f * (zk.y + zn.y), -0.5f * (zk.x - zn.x));
-    const float2 wo = cmul(o, t.twiddle[k]);
-    const float re = e.x + wo.x, im = e.y + wo.y;
-    P[k] = re * re + im * im;
+    const float2 X = rfft_bin<NFFT>(z, t.twiddle, k);
+    P[k] = X.x * X.x + X.y * X.y;
   }
   __syncthreads();
   if (threadIdx.x < NMELS) {
@@ -207,12 +191,88 @@ double mel_to_hz(double m) {
   return m >= min_log_mel ? min_log_hz * std::exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
-struct OnsetTableSet {
-  OnsetTables t;
-  void* dev = nullptr;
-};
-std::mutex g_onset_mu;
-std::map<std::tuple<int, int, int>, OnsetTableSet> g_onset_tables;  // (device, sr, hop)
+// one device allocation holding the given host blocks back to back; *dev points at the first
+cudaError_t upload_blocks(std::initializer_list<std::pair<const void*, size_t>> blocks, char** dev) {
+  size_t total = 0;
+  for (const auto& b : blocks) total += b.second;
+  std::vector<char> host(total);
+  size_t at = 0;
+  for (const auto& b : blocks) { if (b.second) memcpy(host.data() + at, b.first, b.second); at += b.second; }
+  cudaError_t e = cudaMalloc(dev, total);
+  if (e != cudaSuccess) return e;
+  e = cudaMemcpy(*dev, host.data(), total, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { cudaFree(*dev); *dev = nullptr; }
+  return e;
+}
+
+std::mutex g_onset_mu;  // guards the three caches below
+std::map<std::tuple<int, int, int>, OnsetTables> g_onset_tables;  // (device, sr, hop)
+std::map<std::pair<int, int>, FftTables> g_fft_tables;           // (device, n_fft)
+std::map<std::tuple<int, int, int, int, double, double>, MelBank> g_mel_banks;  // (device, sr, n_fft, n_mels, fmin, fmax)
+
+cudaError_t fft_tables_locked(int dev, int n_fft, FftTables* out) {
+  auto it = g_fft_tables.find({dev, n_fft});
+  if (it != g_fft_tables.end()) { *out = it->second; return cudaSuccess; }
+  // twiddles exp(-2 pi i k / n_fft), k = 0..n_fft/2, and the periodic Hann window, both computed in float64
+  const int nbins = n_fft / 2 + 1;
+  std::vector<float2> tw(nbins);
+  for (int k = 0; k < nbins; ++k) {
+    const double a = 2.0 * M_PI * k / n_fft;
+    tw[k] = make_float2((float)std::cos(a), (float)-std::sin(a));
+  }
+  std::vector<float> win(n_fft);
+  for (int k = 0; k < n_fft; ++k) win[k] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * k / n_fft));
+  char* p = nullptr;
+  const size_t b_tw = sizeof(float2) * nbins;
+  cudaError_t e = upload_blocks({{tw.data(), b_tw}, {win.data(), sizeof(float) * n_fft}}, &p);
+  if (e != cudaSuccess) return e;
+  FftTables t;
+  t.twiddle = reinterpret_cast<const float2*>(p);
+  t.window = reinterpret_cast<const float*>(p + b_tw);
+  g_fft_tables[{dev, n_fft}] = t;
+  *out = t;
+  return cudaSuccess;
+}
+
+cudaError_t mel_filterbank_locked(int dev, int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out) {
+  const auto key = std::make_tuple(dev, sr, n_fft, n_mels, fmin, fmax);
+  auto it = g_mel_banks.find(key);
+  if (it != g_mel_banks.end()) { *out = it->second; return cudaSuccess; }
+  // librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm="slaney", dtype=float32)
+  const int nbins = n_fft / 2 + 1;
+  std::vector<double> mel_f(n_mels + 2), fft_f(nbins);
+  const double m0 = hz_to_mel(fmin), m1 = hz_to_mel(fmax), mstep = (m1 - m0) / (n_mels + 1);
+  for (int i = 0; i < n_mels + 2; ++i) mel_f[i] = mel_to_hz(i == n_mels + 1 ? m1 : m0 + i * mstep);  // np.linspace
+  for (int k = 0; k < nbins; ++k) fft_f[k] = k / (n_fft * (1.0 / sr));                             // np.fft.rfftfreq
+  std::vector<float> wpack, row(nbins);
+  std::vector<int32_t> off(n_mels + 1), lo(n_mels);
+  for (int m = 0; m < n_mels; ++m) {
+    const double enorm = 2.0 / (mel_f[m + 2] - mel_f[m]);
+    int first = -1, last = -1;
+    for (int k = 0; k < nbins; ++k) {
+      const double lower = -(mel_f[m] - fft_f[k]) / (mel_f[m + 1] - mel_f[m]);
+      const double upper = (mel_f[m + 2] - fft_f[k]) / (mel_f[m + 2] - mel_f[m + 1]);
+      const float w = (float)std::max(0.0, std::min(lower, upper));
+      row[k] = (float)((double)w * enorm);
+      if (row[k] != 0.f) { if (first < 0) first = k; last = k; }
+    }
+    off[m] = (int32_t)wpack.size();
+    lo[m] = first < 0 ? 0 : first;
+    if (first >= 0) wpack.insert(wpack.end(), row.begin() + first, row.begin() + last + 1);
+  }
+  off[n_mels] = (int32_t)wpack.size();
+  const size_t b_w = sizeof(float) * wpack.size(), b_off = sizeof(int32_t) * (n_mels + 1);
+  char* p = nullptr;
+  cudaError_t e = upload_blocks({{wpack.data(), b_w}, {off.data(), b_off}, {lo.data(), sizeof(int32_t) * n_mels}}, &p);
+  if (e != cudaSuccess) return e;
+  MelBank b;
+  b.w = reinterpret_cast<const float*>(p);
+  b.off = reinterpret_cast<const int32_t*>(p + b_w);
+  b.lo = reinterpret_cast<const int32_t*>(p + b_w + b_off);
+  g_mel_banks[key] = b;
+  *out = b;
+  return cudaSuccess;
+}
 }  // namespace
 
 OnsetGeometry onset_geometry(int sr, int hop) {
@@ -227,6 +287,22 @@ OnsetGeometry onset_geometry(int sr, int hop) {
   return g;
 }
 
+cudaError_t fft_tables(int n_fft, FftTables* out) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lock(g_onset_mu);
+  return fft_tables_locked(dev, n_fft, out);
+}
+
+cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> lock(g_onset_mu);
+  return mel_filterbank_locked(dev, sr, n_fft, n_mels, fmin, fmax, out);
+}
+
 cudaError_t onset_tables(int sr, int hop, OnsetTables* out) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -234,64 +310,23 @@ cudaError_t onset_tables(int sr, int hop, OnsetTables* out) {
   std::lock_guard<std::mutex> lock(g_onset_mu);
   auto key = std::make_tuple(dev, sr, hop);
   auto it = g_onset_tables.find(key);
-  if (it != g_onset_tables.end()) { *out = it->second.t; return cudaSuccess; }
-  // twiddles exp(-2 pi i k / 2048), k = 0..1024, and the periodic Hann window, both computed in float64
-  std::vector<float2> tw(NBINS);
-  for (int k = 0; k < NBINS; ++k) {
-    const double a = 2.0 * M_PI * k / NFFT;
-    tw[k] = make_float2((float)std::cos(a), (float)-std::sin(a));
-  }
-  std::vector<float> win(NFFT);
-  for (int k = 0; k < NFFT; ++k) win[k] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * k / NFFT));
-  // librosa.filters.mel(sr, n_fft=2048, n_mels=128, fmin=0, fmax=sr/2, htk=False, norm="slaney", dtype=float32)
-  std::vector<double> mel_f(NMELS + 2), fft_f(NBINS);
-  const double m0 = hz_to_mel(0.0), m1 = hz_to_mel(0.5 * sr), mstep = (m1 - m0) / (NMELS + 1);
-  for (int i = 0; i < NMELS + 2; ++i) mel_f[i] = mel_to_hz(i == NMELS + 1 ? m1 : m0 + i * mstep);  // np.linspace
-  for (int k = 0; k < NBINS; ++k) fft_f[k] = k / (NFFT * (1.0 / sr));                           // np.fft.rfftfreq
-  std::vector<float> wpack;
-  std::vector<int32_t> off(NMELS + 1), lo(NMELS);
-  for (int m = 0; m < NMELS; ++m) {
-    const double enorm = 2.0 / (mel_f[m + 2] - mel_f[m]);
-    std::vector<float> row(NBINS);
-    int first = -1, last = -1;
-    for (int k = 0; k < NBINS; ++k) {
-      const double lower = -(mel_f[m] - fft_f[k]) / (mel_f[m + 1] - mel_f[m]);
-      const double upper = (mel_f[m + 2] - fft_f[k]) / (mel_f[m + 2] - mel_f[m + 1]);
-      const float w = (float)std::max(0.0, std::min(lower, upper));
-      row[k] = (float)((double)w * enorm);
-      if (row[k] != 0.f) { if (first < 0) first = k; last = k; }
-    }
-    off[m] = (int32_t)wpack.size();
-    lo[m] = first < 0 ? 0 : first;
-    if (first >= 0) wpack.insert(wpack.end(), row.begin() + first, row.begin() + last + 1);
-  }
-  off[NMELS] = (int32_t)wpack.size();
-  const size_t b_tw = sizeof(float2) * NBINS, b_win = sizeof(float) * NFFT, b_w = sizeof(float) * wpack.size(),
-               b_off = sizeof(int32_t) * (NMELS + 1), b_lo = sizeof(int32_t) * NMELS;
-  char* p = nullptr;
-  e = cudaMalloc(&p, b_tw + b_win + b_w + b_off + b_lo);
-  if (e != cudaSuccess) return e;
-  OnsetTableSet s;
-  s.dev = p;
-  s.t.twiddle = reinterpret_cast<const float2*>(p);
-  s.t.window = reinterpret_cast<const float*>(p + b_tw);
-  s.t.mel_w = reinterpret_cast<const float*>(p + b_tw + b_win);
-  s.t.mel_off = reinterpret_cast<const int32_t*>(p + b_tw + b_win + b_w);
-  s.t.mel_lo = reinterpret_cast<const int32_t*>(p + b_tw + b_win + b_w + b_off);
-  std::vector<char> host(b_tw + b_win + b_w + b_off + b_lo);
-  memcpy(host.data(), tw.data(), b_tw);
-  memcpy(host.data() + b_tw, win.data(), b_win);
-  memcpy(host.data() + b_tw + b_win, wpack.data(), b_w);
-  memcpy(host.data() + b_tw + b_win + b_w, off.data(), b_off);
-  memcpy(host.data() + b_tw + b_win + b_w + b_off, lo.data(), b_lo);
-  e = cudaMemcpy(p, host.data(), host.size(), cudaMemcpyHostToDevice);  // once per (device, sr, hop)
-  if (e != cudaSuccess) { cudaFree(p); return e; }
+  if (it != g_onset_tables.end()) { *out = it->second; return cudaSuccess; }
+  FftTables f;
+  MelBank m;
+  if ((e = fft_tables_locked(dev, NFFT, &f)) != cudaSuccess) return e;
+  if ((e = mel_filterbank_locked(dev, sr, NFFT, NMELS, 0.0, 0.5 * sr, &m)) != cudaSuccess) return e;
+  OnsetTables t;
+  t.twiddle = f.twiddle;
+  t.window = f.window;
+  t.mel_w = m.w;
+  t.mel_off = m.off;
+  t.mel_lo = m.lo;
   const OnsetGeometry g = onset_geometry(sr, hop);
-  s.t.pre_max = g.pre_max; s.t.post_max = g.post_max; s.t.pre_avg = g.pre_avg; s.t.post_avg = g.post_avg;
-  s.t.wait = g.wait; s.t.pad = g.pad;
-  s.t.delta = 0.07f;
-  g_onset_tables[key] = s;
-  *out = s.t;
+  t.pre_max = g.pre_max; t.post_max = g.post_max; t.pre_avg = g.pre_avg; t.post_avg = g.post_avg;
+  t.wait = g.wait; t.pad = g.pad;
+  t.delta = 0.07f;
+  g_onset_tables[key] = t;
+  *out = t;
   return cudaSuccess;
 }
 
