@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from oracle import beat_oracle as bo
+from oracle import mel_oracle as mo
 from oracle import onset_oracle as oo
 from oracle import pitch_oracle as po
 from tests import test_gpu_beat_ops as B
@@ -150,3 +151,14 @@ def test_onset_geometry_corners():
     assert {sr for sr, _, _ in O.CASES} >= {8000, 16000, 22050, 44100, 48000, 96000}
     assert {h for _, h, _ in O.CASES} >= {32, 64, 256, 512, 768, 1024, 1025, 1323, 1324, 2048, 4096}
     assert oo.peak_params(44100, 32)["wait"] == 41
+
+
+def test_mel_bits_cases_cover_every_window_and_empty_bands():
+    spec = list(AB.MEL_SPEC_CASES.values())
+    assert {w for w, *_ in spec} == {32, 64, 128, 256, 512, 1024, 2048, 4096}
+    assert any((mo.mel_filterbank(sr, m, w) == 0).all(1).any() for w, _, m, sr, _ in spec)
+    assert any(N == w // 2 + 1 for w, *_, N in spec)
+    for sr, _, _, _, scales in AB.MEL_LOSS_CASES.values():
+        if scales == mo.SEVEN_SCALES:
+            assert sr == 48000 and any((mo.mel_filterbank(sr, m, w) == 0).all(1).any() for m, _, _, w in scales)
+    assert any(scales == mo.DEFAULT_SCALES for *_, scales in AB.MEL_LOSS_CASES.values())

@@ -1,7 +1,8 @@
 """GPU: the audio kernels reproduce, bit for bit, the outputs recorded in tests/golden/audio_bits.npz by
 tools/audio_bits.py: the pitch shift's fp32 output and its four float64 intermediates (spectrum, stretched spectrum,
 inverse-DFT frames, overlap-added signal) at eight parameter points, the beat tracker's envelope, tempo and beats at
-three tempo windows, and the onset detector's envelope and onsets at three (sr, hop).  Schedule, tiling and the order
+three tempo windows, the onset detector's envelope and onsets at three (sr, hop), the mel spectrogram at every window
+length, and the mel loss and per-item losses at two scale sets.  Schedule, tiling and the order
 of stores may change; the float operations on every output and their order may not."""
 import os
 

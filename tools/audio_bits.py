@@ -1,5 +1,5 @@
 """Bit-level record of the audio kernels (vnb_pitch_shift and its float64 intermediates, vnb_beat_track,
-vnb_onset_detect) on seeded inputs:
+vnb_onset_detect, vnb_mel_spectrogram, vnb_mel_loss) on seeded inputs:
 
     python tools/audio_bits.py --write tests/golden/audio_bits.npz
 
@@ -13,7 +13,10 @@ The pitch cases store the fp32 output and the four intermediates that vnb_dbg_pi
 (spectrum, stretched spectrum, inverse-DFT frames, overlap-added signal); they cover odd and even n_fft, the three
 stages isolated (rate 1 with new_freq = sr, the vocoder alone, the resampler alone) and the full composition.  The
 beat cases store the envelope, tempo and beat frames at three tempo-window sizes W, the onset cases the envelope and
-onset frames at three (sr, hop).  The library wrappers here are shared with tests/test_gpu_pitch_ops.py,
+onset frames at three (sr, hop).  The mel spectrogram cases store the spectrogram at every window length from 32 to
+4096, with empty Slaney bands at 48 kHz and one clip of the shortest accepted length; the mel loss cases store the
+loss and the per-item losses of the default two scales and of seven scales at 48 kHz (empty bands at 32 and 64).  The
+library wrappers here are shared with tests/test_gpu_pitch_ops.py,
 tests/test_gpu_beat_ops.py and tests/test_gpu_onset_ops.py.
 """
 from __future__ import annotations
@@ -32,6 +35,7 @@ if ROOT not in sys.path:
 
 from oracle import beat_oracle as bo  # noqa: E402
 from oracle import gen_pitch_golden as gg  # noqa: E402
+from oracle import mel_oracle as mo  # noqa: E402
 from oracle import onset_oracle as oo  # noqa: E402
 from oracle import pitch_oracle as po  # noqa: E402
 from tools.gemm_bits import digest, lib, sample_index  # noqa: E402
@@ -120,6 +124,27 @@ def onset_detect(y, sr, hop, backtrack=True):
     return r.envelope.cpu(), [r.frames[b, :int(counts[b])].cpu() for b in range(counts.numel())]
 
 
+def mel_spectrogram(x, sr, n_fft, hop, n_mels):
+    """vnb_mel_spectrogram on x (rows, N) float32, fmin 0 and fmax sr / 2: (rows, n_mels, F) fp32 on the CPU."""
+    L = lib()
+    xd = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).cuda()
+    rows, N = xd.shape
+    sc = L.MelScale(n_fft, hop, n_mels, 0.0, sr / 2)
+    out = torch.empty(rows, n_mels, 1 + N // hop, dtype=torch.float32, device="cuda")
+    L.check(L.lib().vnb_mel_spectrogram(L.ptr(xd), rows, N, sr, ctypes.byref(sc), L.ptr(out), L.stream_ptr()))
+    return out.cpu()
+
+
+def mel_loss(x, y, sr, scales):
+    """MelSpectrogramLoss over (n_mels, fmin, fmax, window) scales on (B, C, N) float32 pairs: (loss (1,), items (B,))."""
+    from vampnet_b200.audio import AudioSignal
+    from vampnet_b200.metrics import MelSpectrogramLoss
+    m, lo, hi, w = zip(*scales)
+    fn = MelSpectrogramLoss(n_mels=list(m), window_lengths=list(w), mel_fmin=list(lo), mel_fmax=list(hi))
+    xs, ys = (AudioSignal(torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).cuda(), sr) for a in (x, y))
+    return fn(xs, ys).reshape(1).cpu(), fn.per_item(xs, ys).cpu()
+
+
 # ---------------------------------------------------------------------------------------------------- record
 PITCH_CASES = {  # name: rows, N, sr, new_freq, rate, n_fft, hop
     "pitch_n16_h1": (1, 200, 44100, 44100, 1.0, 16, 1),
@@ -141,7 +166,21 @@ ONSET_CASES = {  # name: sr, hop, signal
     "onset_22050_h1324": (22050, 1324, "bursts"),
     "onset_96000_h4096": (96000, 4096, "bursts"),
 }
-CASES = list(PITCH_CASES) + list(BEAT_CASES) + list(ONSET_CASES)
+MEL_SPEC_CASES = {  # name: n_fft, hop, n_mels, sr, N; rows: mo.test_pair's two signals
+    "melspec_w32_sr48000": (32, 8, 5, 48000, 2000),  # band 0 is empty
+    "melspec_w64_sr48000": (64, 16, 10, 48000, 3000),  # an empty band
+    "melspec_w128": (128, 32, 20, 16000, 3000),
+    "melspec_w256": (256, 64, 40, 22050, 5000),
+    "melspec_w512_Nmin": (512, 128, 80, 44100, 257),  # N = n_fft / 2 + 1: the reflection reaches the far end
+    "melspec_w1024": (1024, 256, 160, 48000, 9000),
+    "melspec_w2048": (2048, 512, 150, 44100, 20000),
+    "melspec_w4096": (4096, 1000, 128, 44100, 30000),  # a hop that does not divide N
+}
+MEL_LOSS_CASES = {  # name: sr, N, B, C, scales; item b is mo.test_pair at seed b
+    "mel_loss_default": (44100, 22050, 3, 1, mo.DEFAULT_SCALES),
+    "mel_loss_seven_sr48000": (48000, 12000, 2, 2, mo.SEVEN_SCALES),
+}
+CASES = list(PITCH_CASES) + list(BEAT_CASES) + list(ONSET_CASES) + list(MEL_SPEC_CASES) + list(MEL_LOSS_CASES)
 
 
 def run_named(name):
@@ -158,6 +197,13 @@ def run_named(name):
         sr, hop, sig = ONSET_CASES[name]
         env, onsets = onset_detect(oo.test_signal(sig, sr)[None], sr, hop)
         return [env, onsets[0]]
+    if name in MEL_SPEC_CASES:
+        n_fft, hop, n_mels, sr, N = MEL_SPEC_CASES[name]
+        return [mel_spectrogram(np.concatenate(mo.test_pair(N, sr, seed=11)), sr, n_fft, hop, n_mels)]
+    if name in MEL_LOSS_CASES:
+        sr, N, B, C, scales = MEL_LOSS_CASES[name]
+        pairs = [mo.test_pair(N, sr, seed=b, channels=C) for b in range(B)]
+        return list(mel_loss(np.stack([p[0] for p in pairs]), np.stack([p[1] for p in pairs]), sr, scales))
     raise KeyError(name)
 
 

@@ -224,3 +224,12 @@ def ptr(t):
 def stream_ptr(device=None):
     import torch
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def workspace(device, query, *args):
+    """(workspace, size): a uint8 tensor on ``device`` of the size in bytes that ``query``, one of the
+    ``vnb_*_workspace_bytes`` entry points, reports for ``args``."""
+    import torch
+    n = C.c_uint64(0)
+    check(query(*args, C.byref(n)))
+    return torch.empty(n.value, dtype=torch.uint8, device=device), n.value

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .onset import as_rows
 
 
 class Beats(NamedTuple):
@@ -28,31 +29,22 @@ class Beats(NamedTuple):
 def beat_track(samples: torch.Tensor, sample_rate: int, hop_length: int = 512, start_bpm: float = 120.0,
                tightness: float = 100.0, trim: bool = True) -> Beats:
     """Beats of every row of ``samples`` ((N,) or (B, N) float32 on a CUDA device), each row analysed on its own."""
-    if not torch.is_tensor(samples) or samples.dtype != torch.float32:
-        raise RuntimeError(f"beat_track: samples must be a float32 tensor, got {getattr(samples, 'dtype', type(samples))}")
-    if samples.device.type != "cuda":
-        raise RuntimeError(f"beat_track: samples must be on a CUDA device, got {samples.device}")
-    if samples.ndim == 1:
-        samples = samples[None]
-    if samples.ndim != 2:
-        raise RuntimeError(f"beat_track: samples must be (N,) or (B, N), got {tuple(samples.shape)}")
-    samples = samples.contiguous()
+    samples = as_rows(samples, "beat_track")
     B, N = samples.shape
     L = _lib.lib()
     hop = int(hop_length)
     F = 1 + N // hop if hop > 0 else 1
     dev = samples.device
-    ws_bytes = _lib.C.c_uint64(0)
-    if B > 0 and N > 0 and hop > 0:
-        _lib.check(L.vnb_beat_workspace_bytes(B, N, hop, _lib.C.byref(ws_bytes)))
+    # out-of-range shapes go straight to vnb_beat_track, which names them
+    workspace, ws_bytes = (_lib.workspace(dev, L.vnb_beat_workspace_bytes, B, N, hop) if B > 0 and N > 0 and hop > 0
+                           else (None, 0))
     with torch.cuda.device(dev):
-        workspace = torch.empty(max(int(ws_bytes.value), 1), dtype=torch.uint8, device=dev)
         frames = torch.empty(max(B, 1), F, dtype=torch.int32, device=dev)
         counts = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
         tempo = torch.empty(max(B, 1), dtype=torch.float64, device=dev)
         envelope = torch.empty(max(B, 1), F, dtype=torch.float32, device=dev)
         _lib.check(L.vnb_beat_track(_lib.ptr(samples), B, N, int(sample_rate), hop, float(start_bpm), float(tightness),
-                                    int(bool(trim)), _lib.ptr(workspace), ws_bytes.value, _lib.ptr(envelope),
+                                    int(bool(trim)), _lib.ptr(workspace), ws_bytes, _lib.ptr(envelope),
                                     _lib.ptr(tempo), _lib.ptr(frames), _lib.ptr(counts), _lib.stream_ptr(dev)))
     return Beats(frames, counts, tempo, envelope)
 

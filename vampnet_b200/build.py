@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libvampnet_b200.so")
-SOURCES = ["api.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "elementwise.cu", "sampler.cu", "codec.cu", "conv_wgmma.cu", "lora.cu", "onset.cu", "beat.cu", "pitch.cu", "validate.cu", "mel.cu"]
+SOURCES = ["api.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "elementwise.cu", "sampler.cu", "codec.cu", "conv_wgmma.cu", "lora.cu", "onset.cu", "beat.cu", "pitch.cu", "validate.cu", "mel.cu", "tables.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 

@@ -1224,10 +1224,17 @@ int32_t vnb_dbg_gemm_sample_split(const void* A, const void* W, const float* bia
   return 0;
 }
 
+// the refusal of a caller's workspace that is too small for the call
+static int32_t check_workspace(const char* fn, uint64_t have, uint64_t need) {
+  if (have < need)
+    return fail("%s: workspace of %llu bytes, %llu needed", fn, (unsigned long long)have, (unsigned long long)need);
+  return 0;
+}
+
 // ---- onset detection (onset.cu) ----
 int32_t vnb_onset_workspace_bytes(int32_t B, int32_t N, int32_t hop, uint64_t* bytes) {
   if (B < 1 || N < 1 || hop < 1 || !bytes) return fail("vnb_onset_workspace_bytes: need B >= 1, N >= 1, hop >= 1 and bytes");
-  *bytes = (uint64_t)B * (uint64_t)(1 + N / hop) * 128u * sizeof(float);
+  *bytes = onset_workspace_bytes(B, 1 + N / hop);
   return 0;
 }
 int32_t vnb_onset_detect(const float* samples, int32_t B, int32_t N, int32_t sr, int32_t hop, int32_t backtrack,
@@ -1237,11 +1244,8 @@ int32_t vnb_onset_detect(const float* samples, int32_t B, int32_t N, int32_t sr,
   if (sr < 1 || hop < 1) return fail("vnb_onset_detect: need sr >= 1 and hop >= 1 (got sr = %d, hop = %d)", sr, hop);
   if (!samples || !workspace || !envelope || !onsets || !counts)
     return fail("vnb_onset_detect: samples, workspace, envelope, onsets and counts are required");
-  uint64_t need = 0;
-  vnb_onset_workspace_bytes(B, N, hop, &need);
-  if (workspace_bytes < need)
-    return fail("vnb_onset_detect: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
-                (unsigned long long)need);
+  if (int32_t rc = check_workspace("vnb_onset_detect", workspace_bytes, onset_workspace_bytes(B, 1 + N / hop)))
+    return rc;
   OnsetTables t;
   CK(onset_tables(sr, hop, &t));
   CK(launch_onset_detect(samples, B, N, hop, t, reinterpret_cast<float*>(workspace), envelope, onsets, counts,
@@ -1273,10 +1277,7 @@ static int32_t beat_args(const char* fn, int32_t B, int32_t F, int32_t sr, int32
   const int W = beat_lags(sr, hop);
   if (W < 2 || W > BEAT_MAX_LAGS)
     return fail("%s: the 8 s tempo window is int(8 sr) // hop = %d frames; 2..%d are supported", fn, W, BEAT_MAX_LAGS);
-  const uint64_t need = beat_workspace_bytes(B, F);
-  if (workspace_bytes < need)
-    return fail("%s: workspace of %llu bytes, %llu needed", fn, (unsigned long long)workspace_bytes,
-                (unsigned long long)need);
+  if (int32_t rc = check_workspace(fn, workspace_bytes, beat_workspace_bytes(B, F))) return rc;
   CK(beat_tables(sr, hop, t));
   return 0;
 }
@@ -1339,10 +1340,7 @@ int32_t vnb_pitch_shift(const float* samples, int32_t rows, int32_t N, int32_t s
   if (!samples || !workspace || !out) return fail("vnb_pitch_shift: samples, workspace and out are required");
   PitchPlan p;
   if (int32_t rc = pitch_args("vnb_pitch_shift", rows, N, sr, new_freq, n_fft, hop, rate, &p)) return rc;
-  const uint64_t need = pitch_workspace_bytes(p);
-  if (workspace_bytes < need)
-    return fail("vnb_pitch_shift: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
-                (unsigned long long)need);
+  if (int32_t rc = check_workspace("vnb_pitch_shift", workspace_bytes, pitch_workspace_bytes(p))) return rc;
   const double *fwd = nullptr, *inv = nullptr;
   CK(pitch_basis(n_fft, &fwd, &inv));
   CK(launch_pitch_shift(samples, p, fwd, inv, workspace, out, reinterpret_cast<cudaStream_t>(stream)));
@@ -1391,9 +1389,7 @@ int32_t vnb_xent_metrics(const float* logits, const int64_t* z, const int64_t* m
   if (!(label_smoothing >= 0.0 && label_smoothing <= 1.0))
     return fail("vnb_xent_metrics: need 0 <= label_smoothing <= 1 (got %g)", label_smoothing);
   const uint64_t need = xent_workspace_bytes(B, (long long)T * (C - ncc));
-  if (workspace_bytes < need)
-    return fail("vnb_xent_metrics: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
-                (unsigned long long)need);
+  if (int32_t rc = check_workspace("vnb_xent_metrics", workspace_bytes, need)) return rc;
   CK(launch_xent_metrics(logits, z, mask, r, B, C, T, ncc, V, label_smoothing, workspace, out9, ambiguous,
                          reinterpret_cast<cudaStream_t>(stream)));
   return 0;
@@ -1455,9 +1451,7 @@ int32_t vnb_mel_loss(const float* x, const float* y, int32_t B, int32_t C, int32
   if (!std::isfinite(pow) || !std::isfinite(log_weight) || !std::isfinite(mag_weight))
     return fail("vnb_mel_loss: pow, log_weight and mag_weight must be finite");
   const MelLossPlan p = mel_loss_plan(B, C, N, sr, scales, n_scales);
-  if (workspace_bytes < p.total)
-    return fail("vnb_mel_loss: workspace of %llu bytes, %llu needed", (unsigned long long)workspace_bytes,
-                (unsigned long long)p.total);
+  if (int32_t rc = check_workspace("vnb_mel_loss", workspace_bytes, p.total)) return rc;
   CK(launch_mel_loss(x, y, p, clamp_eps, pow, log_weight, mag_weight, workspace, loss, item_loss,
                      reinterpret_cast<cudaStream_t>(stream)));
   return 0;

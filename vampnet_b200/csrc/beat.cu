@@ -1,7 +1,7 @@
 // vampnet_b200 — beat tracking for the beat-synced mask (reference vampnet/interface.py:226-322 takes its beat times
 // from WaveBeat; this is librosa 0.10.1's beat.beat_track(y, sr, hop_length=H) restated instead), all on one stream
 // with no host round trip:
-//   onset_spec_kernel      (onset.cu, unchanged) the fp32 mel dB spectrogram
+//   mel_spec_kernel        (mel.cu, ONSET_DB mode, as onset detection runs it) the fp32 mel dB spectrogram
 //   beat_floor_kernel      one CTA per row: the clip's dB maximum minus top_db = 80
 //   beat_flux_kernel       one warp per (frame, row): the clamped spectral flux of the 128 bands and its median (the
 //                          mean of the 64th and 65th smallest), shifted by the envelope's padding: the fp32 envelope
@@ -11,43 +11,20 @@
 //   beat_track_kernel      one CTA per row: the mean tempogram, the prior and the tempo argmax; the envelope over its
 //                          standard deviation and the Gaussian local score; the dynamic programme (one warp, the best
 //                          of ~1.5 period predecessors per frame); the last beat, the backtrack and the trim
-// DESIGN.md §10 has the numerics; oracle/beat_oracle.py restates the algorithm in float64.
+// DESIGN.md §10 has the numerics; oracle/beat_oracle.py restates the algorithm in float64.  The tables (window, tempo
+// frequencies) are built here on the host and cached by device_table.
 #include <cfloat>
 #include <climits>
 #include <cmath>
-#include <cstring>
-#include <map>
-#include <mutex>
-#include <tuple>
-#include <vector>
 
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace vnb {
 
 namespace {
-constexpr int NMELS = 128, THREADS = 256, WARPS = THREADS / 32;
+constexpr int NMELS = ONSET_NMELS, THREADS = 256, WARPS = THREADS / 32;
 constexpr int MAXG = 2 * BEAT_MAX_LAGS;  // Gaussian taps (2 period + 1) and DP candidates, period <= W - 1
-
-__device__ double block_sum(double v, double* red) {
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();  // red[] may still be read by a previous reduction
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  v = red[0];
-  for (int w = 1; w < WARPS; ++w) v += red[w];
-  return v;
-}
-
-__device__ double block_max(double v, double* red) {
-  for (int o = 16; o; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  v = red[0];
-  for (int w = 1; w < WARPS; ++w) v = fmax(v, red[w]);
-  return v;
-}
 
 // (value, index) with the larger value, the smaller index on a tie: numpy's argmax keeps the first maximum
 __device__ __forceinline__ void arg_better(double& v, int& i, double ov, int oi) {
@@ -63,7 +40,7 @@ __global__ void __launch_bounds__(THREADS) beat_floor_kernel(const float* __rest
   const float* d = db + (size_t)blockIdx.x * F * NMELS;
   float mx = -INFINITY;
   for (size_t i = threadIdx.x; i < (size_t)F * NMELS; i += THREADS) mx = fmaxf(mx, d[i]);
-  mx = (float)block_max((double)mx, red);  // exact: a float's maximum
+  mx = (float)block_reduce<Reduce::MAX, WARPS>((double)mx, red);  // exact: a float's maximum
   if (threadIdx.x == 0) floor_db[blockIdx.x] = mx - 80.f;
 }
 
@@ -138,7 +115,8 @@ __global__ void __launch_bounds__(THREADS) beat_tempogram_kernel(const float* __
       ac[r] = s;
       mx = fmax(mx, fabs(s));
     }
-    mx = block_max(mx, red);  // also orders this frame's reads of a[] before the next frame's writes
+    // also orders this frame's reads of a[] before the next frame's writes
+    mx = block_reduce<Reduce::MAX, WARPS>(mx, red);
     if (mx < DBL_MIN) mx = 1.0;  // util.normalize leaves a frame below tiny(float64) as it is
 #pragma unroll
     for (int r = 0; r < LAGS_PER_THREAD; ++r) acc[r] += ac[r] / mx;
@@ -217,10 +195,10 @@ __global__ void __launch_bounds__(THREADS) beat_track_kernel(const float* __rest
   // ---- local score: the envelope over its standard deviation (ddof = 1), convolved with a Gaussian
   double sum = 0.0;
   for (int i = threadIdx.x; i < F; i += THREADS) sum += e[i];
-  const double mean = block_sum(sum, red) / F;
+  const double mean = block_reduce<Reduce::SUM, WARPS>(sum, red) / F;
   double sq = 0.0;
   for (int i = threadIdx.x; i < F; i += THREADS) sq += ((double)e[i] - mean) * ((double)e[i] - mean);
-  sq = block_sum(sq, red);
+  sq = block_reduce<Reduce::SUM, WARPS>(sq, red);
   const double norm = F > 1 ? sqrt(sq / (F - 1)) : NAN;
   for (int i = threadIdx.x; i < F; i += THREADS) x[i] = norm > 0 ? (double)e[i] / norm : (double)e[i];
   for (int j = threadIdx.x; j <= 2 * period; j += THREADS) {
@@ -240,7 +218,8 @@ __global__ void __launch_bounds__(THREADS) beat_track_kernel(const float* __rest
     ls[i] = acc;
     lmax = fmax(lmax, acc);
   }
-  const double thr = 0.01 * block_max(lmax, red);  // also orders the ls[] writes before the reads below
+  // also orders the ls[] writes before the reads below
+  const double thr = 0.01 * block_reduce<Reduce::MAX, WARPS>(lmax, red);
   // ---- dynamic programme: one warp, frame by frame
   if (warp == 0) {
     bool first = true;
@@ -322,15 +301,6 @@ __global__ void __launch_bounds__(THREADS) beat_track_kernel(const float* __rest
   counts[b] = cnt;
 }
 
-struct BeatTableSet {
-  BeatTables t;
-  void* dev = nullptr;
-};
-std::mutex g_beat_mu;
-std::map<std::tuple<int, int, int>, BeatTableSet> g_beat_tables;  // (device, sr, hop)
-
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
 // the workspace, in order: mel dB (B, F, 128) f32, floors (B) f32, tempogram chunk sums, TrackScratch's arrays
 struct BeatLayout {
   size_t db, floor, partial, x, ls, cum, vals, gauss, txwt, back, chain, total;
@@ -338,20 +308,19 @@ struct BeatLayout {
 BeatLayout beat_layout(int B, int F) {
   BeatLayout l;
   size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o = align256(o + bytes); return at; };
   const size_t bf = (size_t)B * F;
-  l.db = take(bf * NMELS * sizeof(float));
-  l.floor = take((size_t)B * sizeof(float));
+  l.db = carve(o, bf * NMELS * sizeof(float));
+  l.floor = carve(o, (size_t)B * sizeof(float));
   // nchunk * W <= (F / fpc + 1) * W <= 256 F + W with fpc = ceil(W / 256)
-  l.partial = take((size_t)B * (256 * (size_t)F + BEAT_MAX_LAGS) * sizeof(double));
-  l.x = take(bf * sizeof(double));
-  l.ls = take(bf * sizeof(double));
-  l.cum = take(bf * sizeof(double));
-  l.vals = take(bf * sizeof(double));
-  l.gauss = take((size_t)B * MAXG * sizeof(double));
-  l.txwt = take((size_t)B * MAXG * sizeof(double));
-  l.back = take(bf * sizeof(int32_t));
-  l.chain = take(bf * sizeof(int32_t));
+  l.partial = carve(o, (size_t)B * (256 * (size_t)F + BEAT_MAX_LAGS) * sizeof(double));
+  l.x = carve(o, bf * sizeof(double));
+  l.ls = carve(o, bf * sizeof(double));
+  l.cum = carve(o, bf * sizeof(double));
+  l.vals = carve(o, bf * sizeof(double));
+  l.gauss = carve(o, (size_t)B * MAXG * sizeof(double));
+  l.txwt = carve(o, (size_t)B * MAXG * sizeof(double));
+  l.back = carve(o, bf * sizeof(int32_t));
+  l.chain = carve(o, bf * sizeof(int32_t));
   l.total = o;
   return l;
 }
@@ -380,47 +349,40 @@ cudaError_t launch_decisions(const float* env, int B, int F, int sr, int hop, co
   count_launch();
   return cudaGetLastError();
 }
+
+// tempo_frequencies: inf, then 60 sr / (hop k)
+double tempo_bpm(int sr, int hop, int k) { return k == 0 ? INFINITY : 60.0 * sr / ((double)hop * k); }
 }  // namespace
 
 int beat_lags(int sr, int hop) { return (int)std::min<long long>(8LL * sr / hop, INT_MAX); }
 
 size_t beat_workspace_bytes(int B, int F) { return beat_layout(B, F).total; }
 
+// one table: the window, the tempo frequencies, their log2 (W doubles each)
 cudaError_t beat_tables(int sr, int hop, BeatTables* out) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  std::lock_guard<std::mutex> lock(g_beat_mu);
-  auto key = std::make_tuple(dev, sr, hop);
-  auto it = g_beat_tables.find(key);
-  if (it != g_beat_tables.end()) { *out = it->second.t; return cudaSuccess; }
   const int W = beat_lags(sr, hop);
   if (W < 2 || W > BEAT_MAX_LAGS) return cudaErrorInvalidValue;
-  // scipy's periodic Hann (0.5 + 0.5 cos of linspace(-pi, pi, W + 1)), tempo_frequencies and their log2, in float64
-  std::vector<double> host(3 * (size_t)W);
-  double *win = host.data(), *bpm = win + W, *l2 = bpm + W;
-  const double step = 2.0 * M_PI / W;
-  int max_idx = -1;
-  for (int k = 0; k < W; ++k) {
-    win[k] = 0.5 + 0.5 * std::cos(k * step + -M_PI);
-    bpm[k] = k == 0 ? INFINITY : 60.0 * sr / ((double)hop * k);
-    l2[k] = std::log2(bpm[k]);
-    if (max_idx < 0 && bpm[k] < 320.0) max_idx = k;
-  }
-  char* p = nullptr;
-  e = cudaMalloc(&p, host.size() * sizeof(double));
+  const char* p = nullptr;
+  cudaError_t e = device_table({TABLE_BEAT, (double)sr, (double)hop}, [&] {
+    // scipy's periodic Hann (0.5 + 0.5 cos of linspace(-pi, pi, W + 1)), tempo_frequencies and their log2, in float64
+    std::vector<char> img(3 * sizeof(double) * W);
+    double *win = reinterpret_cast<double*>(img.data()), *bpm = win + W, *l2 = bpm + W;
+    const double step = 2.0 * M_PI / W;
+    for (int k = 0; k < W; ++k) {
+      win[k] = 0.5 + 0.5 * std::cos(k * step + -M_PI);
+      bpm[k] = tempo_bpm(sr, hop, k);
+      l2[k] = std::log2(bpm[k]);
+    }
+    return img;
+  }, &p);
   if (e != cudaSuccess) return e;
-  e = cudaMemcpy(p, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice);  // once per (device, sr, hop)
-  if (e != cudaSuccess) { cudaFree(p); return e; }
-  BeatTableSet s;
-  s.dev = p;
-  s.t.window = reinterpret_cast<const double*>(p);
-  s.t.bpm = s.t.window + W;
-  s.t.log2_bpm = s.t.bpm + W;
-  s.t.W = W;
-  s.t.max_idx = max_idx < 0 ? 0 : max_idx;  // np.argmax of all-False
-  g_beat_tables[key] = s;
-  *out = s.t;
+  out->window = reinterpret_cast<const double*>(p);
+  out->bpm = out->window + W;
+  out->log2_bpm = out->bpm + W;
+  out->W = W;
+  out->max_idx = 0;  // np.argmax of all-False
+  for (int k = 0; k < W; ++k)
+    if (tempo_bpm(sr, hop, k) < 320.0) { out->max_idx = k; break; }
   return cudaSuccess;
 }
 
@@ -432,11 +394,12 @@ cudaError_t launch_beat_track(const float* samples, int B, int N, int sr, int ho
   const BeatLayout l = beat_layout(B, F);
   float* db = reinterpret_cast<float*>(ws + l.db);
   float* floor_db = reinterpret_cast<float*>(ws + l.floor);
-  cudaError_t e = launch_onset_spec(samples, B, N, hop, ot, db, st);
+  cudaError_t e =
+      launch_spectrogram(SpecMode::ONSET_DB, samples, B, N, hop, ONSET_NFFT, ot.fft, ot.bank, NMELS, db, st);
   if (e != cudaSuccess) return e;
   beat_floor_kernel<<<B, THREADS, 0, st>>>(db, F, floor_db);
   count_launch();
-  beat_flux_kernel<<<dim3((F + WARPS - 1) / WARPS, B), THREADS, 0, st>>>(db, F, ot.pad, floor_db, env);
+  beat_flux_kernel<<<dim3((F + WARPS - 1) / WARPS, B), THREADS, 0, st>>>(db, F, ot.g.pad, floor_db, env);
   count_launch();
   return launch_decisions(env, B, F, sr, hop, bt, start_bpm, tightness, trim, ws, tempo, beats, counts, st);
 }

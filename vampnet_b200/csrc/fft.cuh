@@ -1,4 +1,4 @@
-// vampnet_b200 — the fp32 radix-2 real FFT in shared memory that onset.cu and mel.cu share.  An NFFT-point real
+// vampnet_b200 — the fp32 radix-2 real FFT in shared memory of the spectrogram kernel (mel.cu).  An NFFT-point real
 // transform runs as an NFFT/2-point complex FFT of the even/odd sample pairs, then the real split.  Twiddles are
 // twiddle[k] = exp(-2 pi i k / NFFT), k = 0..NFFT/2 (fft_tables()).
 #pragma once

@@ -5,6 +5,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
+#include <vector>
+
 #include "../../include/vampnet_b200.h"
 
 namespace vnb {
@@ -31,6 +34,22 @@ inline int device_sm_count() {
 
 // kernels launched by this library so far (vnb_launch_count; graph replays add their node count)
 void count_launch(unsigned long long n = 1);
+
+// Workspaces and tables are laid out as 256-byte aligned blocks: carve(o, bytes) returns the block's offset o and moves
+// o past it to the next 256-byte boundary, so after the last block o is the total size.
+inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
+inline size_t carve(size_t& o, size_t bytes) {
+  const size_t at = o;
+  o = align256(o + bytes);
+  return at;
+}
+
+// Constant device tables (tables.cu): the table named by `key` (its kind, then the parameters its values depend on) is
+// built on the host by `build` once per (current device, key), uploaded, and kept for the life of the process; *dev
+// receives its device copy.
+enum TableKind { TABLE_FFT, TABLE_MEL_BANK, TABLE_BEAT, TABLE_PITCH_BASIS };
+cudaError_t device_table(const std::vector<double>& key, const std::function<std::vector<char>()>& build,
+                         const char** dev);
 
 // ---- TMA tensor maps (driver entry point fetched at run time; no link-time libcuda dependency) ----
 // 2-D bf16 row-major (rows, cols) with a (box_rows x 64) box, 128B swizzle.
@@ -184,7 +203,7 @@ cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cud
 // groups from `partials`, the nucleus draw the rows of top-p groups from a.logits, then the re-mask
 cudaError_t launch_sample_split_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
 
-// ---- host tables shared by onset.cu and mel.cu: built in float64, rounded to fp32 once, then cached (onset.cu) ----
+// ---- spectrogram tables (mel.cu): built in float64, rounded to fp32 once, cached by device_table ----
 struct FftTables {
   const float2* twiddle;  // (n_fft / 2 + 1) exp(-2 pi i k / n_fft), for fft.cuh
   const float* window;    // (n_fft) periodic Hann
@@ -198,23 +217,31 @@ struct MelBank {
 };
 cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out);  // per (device, all)
 
+// The spectrogram kernel's two outputs from samples (rows, N) fp32, F = 1 + N / hop frames:
+//   ONSET_DB  onset detection's: zero padding (any N >= 1), ONSET_NFFT points, |X|^2 on ONSET_NMELS bands, then
+//             10 log10(max(1e-10, s)); (rows, F, ONSET_NMELS)
+//   MEL_MAG   the mel distance's: reflect padding (N > n_fft / 2), n_fft a power of two in MEL_MIN_NFFT..MEL_MAX_NFFT,
+//             |X| on n_mels bands; (rows, n_mels, F)
+enum class SpecMode { ONSET_DB, MEL_MAG };
+constexpr int ONSET_NFFT = 2048, ONSET_NMELS = 128;
+cudaError_t launch_spectrogram(SpecMode mode, const float* samples, int rows, int N, int hop, int n_fft,
+                               const FftTables& fft, const MelBank& bank, int n_mels, float* out, cudaStream_t st);
+
 // ---- onset detection (onset.cu; librosa 0.10 onset_detect restated, DESIGN.md §9) ----
 // peak_pick windows of onset_detect's defaults at (sr, hop), and the envelope's left padding lag + n_fft // (2 hop)
 struct OnsetGeometry {
   int pre_max = 0, post_max = 0, pre_avg = 0, post_avg = 0, wait = 0, pad = 0;
 };
 OnsetGeometry onset_geometry(int sr, int hop);
-// device tables (built on the host in float64 once per (device, sr, hop), then cached) and the peak_pick parameters
+// the cached FFT tables and Slaney bank at (sr, ONSET_NFFT, ONSET_NMELS), and the peak_pick parameters
 struct OnsetTables {
-  const float2* twiddle;   // (1025) exp(-2 pi i k / 2048)
-  const float* window;     // (2048) periodic Hann
-  const float* mel_w;      // nonzero Slaney mel weights, band m at [mel_off[m], mel_off[m + 1])
-  const int32_t* mel_off;  // (129)
-  const int32_t* mel_lo;   // (128) first nonzero bin of band m
-  int pre_max, post_max, pre_avg, post_avg, wait, pad;
+  FftTables fft;
+  MelBank bank;
+  OnsetGeometry g;
   float delta;
 };
 cudaError_t onset_tables(int sr, int hop, OnsetTables* out);
+size_t onset_workspace_bytes(int B, int F);
 // samples (B, N) fp32 -> db_ws (B, F, 128) mel dB, env (B, F) normalised envelope, onsets (B, F) + counts (B)
 cudaError_t launch_onset_detect(const float* samples, int B, int N, int hop, const OnsetTables& t, float* db_ws,
                                 float* env, int32_t* onsets, int32_t* counts, int backtrack, cudaStream_t st);
@@ -222,15 +249,12 @@ cudaError_t launch_onset_detect(const float* samples, int B, int N, int hop, con
 // onset_rows == 1, else r = b; 1 elsewhere
 cudaError_t launch_onset_mask(const int32_t* onsets, const int32_t* counts, int onset_rows, int F, int width,
                               int64_t* mask, int B, int C, int T, cudaStream_t st);
-// samples (B, N) fp32 -> db (B, F, 128) mel dB: onset_spec_kernel alone (the first half of launch_onset_detect)
-cudaError_t launch_onset_spec(const float* samples, int B, int N, int hop, const OnsetTables& t, float* db,
-                              cudaStream_t st);
 
 // ---- beat tracking (beat.cu; librosa 0.10.1 beat_track restated, DESIGN.md §10) ----
 // the tempo estimate's autocorrelation window, W = int(8 sr) // hop lags, is supported for 2 <= W <= BEAT_MAX_LAGS
 constexpr int BEAT_MAX_LAGS = 4096;
 int beat_lags(int sr, int hop);
-// device tables (float64, built on the host once per (device, sr, hop), then cached)
+// device tables (float64, built on the host once per (device, sr, hop), then cached by device_table)
 struct BeatTables {
   const double* window;    // (W) periodic Hann
   const double* bpm;       // (W) tempo_frequencies: inf, 60 sr / (hop k)
@@ -268,7 +292,7 @@ struct PitchLayout {
 PitchLayout pitch_layout(const PitchPlan& p);
 size_t pitch_workspace_bytes(const PitchPlan& p);
 // float64 forward (n_fft x 2 n_bins) and inverse (2 n_bins x n_fft) DFT bases, zero padded to the GEMM tiles; built on
-// the host once per (device, n_fft), then cached
+// the host once per (device, n_fft), then cached by device_table as one table
 cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv);
 // samples (rows, N) fp32 -> out (rows, N) fp32
 cudaError_t launch_pitch_shift(const float* x, const PitchPlan& p, const double* fwd, const double* inv, void* ws,

@@ -1,16 +1,24 @@
-// vampnet_b200 — mel spectrogram and the multi-scale mel distance of audiotools' MelSpectrogramLoss (the reference's
-// scripts/exp/eval.py scores generated audio with it), all on one stream with no host round trip:
-//   mel_spec_kernel<NFFT>   one CTA per (FPC frames, row): reflect-indexed frame times the periodic Hann window ->
-//                           fp32 NFFT-point real FFT in shared memory (fft.cuh) -> |X| -> each Slaney mel band summed
-//                           over its nonzero bin range; (rows, n_mels, F) fp32
-//   mel_diff_kernel         one CTA per (chunk of MEL_CHUNK elements, item) of one scale: |d log10| and |d| in float64
-//   mel_final_kernel        one CTA: each item's chunk sums in order -> item losses, then the items in order -> loss
-// DESIGN.md §13 has the definition and the numerics; oracle/mel_oracle.py restates it in float64.
+// vampnet_b200 — the spectrogram kernel that onset detection, the beat tracker and the mel distance share, and the
+// multi-scale mel distance of audiotools' MelSpectrogramLoss (the reference's scripts/exp/eval.py scores generated
+// audio with it), all on one stream with no host round trip:
+//   mel_spec_kernel<NFFT, MODE>  one CTA per (FPC frames, row): Hann-windowed frame -> fp32 NFFT-point real FFT in
+//                                shared memory (fft.cuh) -> each Slaney mel band summed over its nonzero bin range.
+//                                ONSET_DB (NFFT 2048; onset.cu, beat.cu): zero padding, |X|^2 on 128 bands, then
+//                                10 log10(max(1e-10, S)); (rows, F, 128).  MEL_MAG: reflect padding, |X|;
+//                                (rows, n_mels, F)
+//   mel_diff_kernel              one CTA per (chunk of MEL_CHUNK elements, item) of one scale: |d log10| and |d| in
+//                                float64
+//   mel_final_kernel             one CTA: each item's chunk sums in order -> item losses, then the items in order ->
+//                                loss
+// The FFT tables and Slaney filterbanks are built here on the host in float64 and cached by device_table.  DESIGN.md
+// §9 and §13 have the numerics; oracle/onset_oracle.py and oracle/mel_oracle.py restate them in float64.
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
 #include "fft.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace vnb {
 
@@ -32,28 +40,35 @@ struct MelSpecArgs {
   int n_mels;
 };
 
-template <int NFFT>
+template <int NFFT, SpecMode MODE>
 __global__ void __launch_bounds__(THREADS) mel_spec_kernel(const float* __restrict__ samples, int N, int F, int hop,
                                                            MelSpecArgs t, float* __restrict__ out) {
+  constexpr bool DB = MODE == SpecMode::ONSET_DB;
   constexpr int NH = NFFT / 2, NBINS = NH + 1, TPF = MelGeom<NFFT>::TPF, FPC = MelGeom<NFFT>::FPC;
   __shared__ float2 zs[FPC * NH];
   __shared__ float Ps[FPC * NBINS];
   const int g = threadIdx.x / TPF, lt = threadIdx.x % TPF;
   const int f = blockIdx.x * FPC + g, row = blockIdx.y;
-  const bool live = f < F;  // the last CTA's spare groups still take part in the block-wide barriers
+  const bool live = FPC == 1 || f < F;  // the last CTA's spare groups still take part in the block-wide barriers
   float2* z = zs + g * NH;
   float* P = Ps + g * NBINS;
   const float* x = samples + (size_t)row * N;
-  const long long s0 = (long long)f * hop - NFFT / 2;  // center=True; N > NFFT / 2, so one reflection reaches
+  const long long s0 = (long long)f * hop - NFFT / 2;  // center=True
   for (int m = lt; m < NH; m += TPF) {
     float a = 0.f, c = 0.f;
     if (live) {
-      long long s = s0 + 2 * m;
-      s = s < 0 ? -s : s >= N ? 2 * (long long)(N - 1) - s : s;
-      long long s1 = s0 + 2 * m + 1;
-      s1 = s1 < 0 ? -s1 : s1 >= N ? 2 * (long long)(N - 1) - s1 : s1;
-      a = x[s] * t.fft.window[2 * m];
-      c = x[s1] * t.fft.window[2 * m + 1];
+      long long s = s0 + 2 * m, s1 = s0 + 2 * m + 1;
+      if (DB) {  // zero padding (pad_mode="constant"), any N
+        a = (s >= 0 && s < N) ? x[s] : 0.f;
+        c = (s1 >= 0 && s1 < N) ? x[s1] : 0.f;
+      } else {  // reflect padding: N > NFFT / 2, so one reflection reaches
+        s = s < 0 ? -s : s >= N ? 2 * (long long)(N - 1) - s : s;
+        s1 = s1 < 0 ? -s1 : s1 >= N ? 2 * (long long)(N - 1) - s1 : s1;
+        a = x[s];
+        c = x[s1];
+      }
+      a *= t.fft.window[2 * m];
+      c *= t.fft.window[2 * m + 1];
     }
     z[__brev(m) >> (32 - ilog2(NH))] = make_float2(a, c);
   }
@@ -61,28 +76,22 @@ __global__ void __launch_bounds__(THREADS) mel_spec_kernel(const float* __restri
   fft_radix2<NFFT>(z, t.fft.twiddle, lt, TPF);
   for (int k = lt; k < NBINS; k += TPF) {
     const float2 X = rfft_bin<NFFT>(z, t.fft.twiddle, k);
-    P[k] = sqrtf(X.x * X.x + X.y * X.y);
+    const float p = X.x * X.x + X.y * X.y;
+    P[k] = DB ? p : sqrtf(p);
   }
   __syncthreads();
   if (!live) return;
-  for (int m = lt; m < t.n_mels; m += TPF) {
+  const int n_mels = DB ? ONSET_NMELS : t.n_mels;
+  for (int m = lt; m < n_mels; m += TPF) {
     const int o0 = t.bank.off[m], o1 = t.bank.off[m + 1];
     const float* p = P + t.bank.lo[m] - o0;
     float s = 0.f;
     for (int o = o0; o < o1; ++o) s = fmaf(t.bank.w[o], p[o], s);
-    out[((size_t)row * t.n_mels + m) * F + f] = s;
+    if (DB)
+      out[((size_t)row * F + f) * ONSET_NMELS + m] = 10.f * log10f(fmaxf(1e-10f, s));
+    else
+      out[((size_t)row * n_mels + m) * F + f] = s;
   }
-}
-
-// fixed-order block sum: a xor tree in each warp, then the warps in order
-__device__ double block_sum(double v, double* red) {
-  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = red[0];
-  for (int w = 1; w < THREADS / 32; ++w) s += red[w];
-  __syncthreads();
-  return s;
 }
 
 // X and Y (B items of `elems` values each) -> partial[b * chunks + c] = (sum |d log10|, sum |d|) over chunk c
@@ -101,8 +110,8 @@ __global__ void __launch_bounds__(THREADS) mel_diff_kernel(const float* __restri
     sl += fabs(pw * log10(fmax(xv, eps)) - pw * log10(fmax(yv, eps)));
     sm += fabs(xv - yv);
   }
-  sl = block_sum(sl, red);
-  sm = block_sum(sm, red);
+  sl = block_reduce<Reduce::SUM, THREADS / 32>(sl, red);
+  sm = block_reduce<Reduce::SUM, THREADS / 32>(sm, red);
   if (threadIdx.x == 0) partial[(size_t)b * chunks + c] = make_double2(sl, sm);
 }
 
@@ -142,22 +151,13 @@ __global__ void __launch_bounds__(THREADS) mel_final_kernel(const double2* __res
   loss[0] = (float)l;
 }
 
-size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
-
-cudaError_t spec_launch(const float* samples, int rows, int N, int F, int hop, const MelSpecArgs& t, float* out,
-                        int n_fft, cudaStream_t st) {
-  switch (n_fft) {
-#define MEL_CASE(NF)                                                                                             \
-  case NF:                                                                                                       \
-    mel_spec_kernel<NF><<<dim3((F + MelGeom<NF>::FPC - 1) / MelGeom<NF>::FPC, rows), THREADS, 0, st>>>(         \
-        samples, N, F, hop, t, out);                                                                             \
-    break;
-    MEL_CASE(32) MEL_CASE(64) MEL_CASE(128) MEL_CASE(256) MEL_CASE(512) MEL_CASE(1024) MEL_CASE(2048) MEL_CASE(4096)
-#undef MEL_CASE
-    default: return cudaErrorInvalidValue;
-  }
-  count_launch();
-  return cudaGetLastError();
+double hz_to_mel(double f) {
+  const double f_sp = 200.0 / 3, min_log_hz = 1000.0, min_log_mel = min_log_hz / f_sp, logstep = std::log(6.4) / 27.0;
+  return f >= min_log_hz ? min_log_mel + std::log(f / min_log_hz) / logstep : f / f_sp;
+}
+double mel_to_hz(double m) {
+  const double f_sp = 200.0 / 3, min_log_hz = 1000.0, min_log_mel = min_log_hz / f_sp, logstep = std::log(6.4) / 27.0;
+  return m >= min_log_mel ? min_log_hz * std::exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
 cudaError_t spec_args(int sr, const vnb_mel_scale& s, MelSpecArgs* t) {
@@ -167,6 +167,93 @@ cudaError_t spec_args(int sr, const vnb_mel_scale& s, MelSpecArgs* t) {
   return mel_filterbank(sr, s.n_fft, s.n_mels, s.fmin, s.fmax, &t->bank);
 }
 }  // namespace
+
+// one table: the twiddles, then the window
+cudaError_t fft_tables(int n_fft, FftTables* out) {
+  const int nbins = n_fft / 2 + 1;
+  const size_t b_tw = sizeof(float2) * nbins;
+  const char* p = nullptr;
+  cudaError_t e = device_table({TABLE_FFT, (double)n_fft}, [&] {
+    // twiddles exp(-2 pi i k / n_fft), k = 0..n_fft/2, and the periodic Hann window, both computed in float64
+    std::vector<char> img(b_tw + sizeof(float) * n_fft);
+    float2* tw = reinterpret_cast<float2*>(img.data());
+    float* win = reinterpret_cast<float*>(img.data() + b_tw);
+    for (int k = 0; k < nbins; ++k) {
+      const double a = 2.0 * M_PI * k / n_fft;
+      tw[k] = make_float2((float)std::cos(a), (float)-std::sin(a));
+    }
+    for (int k = 0; k < n_fft; ++k) win[k] = (float)(0.5 - 0.5 * std::cos(2.0 * M_PI * k / n_fft));
+    return img;
+  }, &p);
+  if (e != cudaSuccess) return e;
+  out->twiddle = reinterpret_cast<const float2*>(p);
+  out->window = reinterpret_cast<const float*>(p + b_tw);
+  return cudaSuccess;
+}
+
+// one table: off, then lo, then the packed weights
+cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out) {
+  const size_t b_off = sizeof(int32_t) * (n_mels + 1), b_lo = sizeof(int32_t) * n_mels;
+  const char* p = nullptr;
+  cudaError_t e = device_table({TABLE_MEL_BANK, (double)sr, (double)n_fft, (double)n_mels, fmin, fmax}, [&] {
+    // librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm="slaney", dtype=float32)
+    const int nbins = n_fft / 2 + 1;
+    std::vector<double> mel_f(n_mels + 2), fft_f(nbins);
+    const double m0 = hz_to_mel(fmin), m1 = hz_to_mel(fmax), mstep = (m1 - m0) / (n_mels + 1);
+    for (int i = 0; i < n_mels + 2; ++i) mel_f[i] = mel_to_hz(i == n_mels + 1 ? m1 : m0 + i * mstep);  // np.linspace
+    for (int k = 0; k < nbins; ++k) fft_f[k] = k / (n_fft * (1.0 / sr));                             // np.fft.rfftfreq
+    std::vector<float> wpack, row(nbins);
+    std::vector<int32_t> off(n_mels + 1), lo(n_mels);
+    for (int m = 0; m < n_mels; ++m) {
+      const double enorm = 2.0 / (mel_f[m + 2] - mel_f[m]);
+      int first = -1, last = -1;
+      for (int k = 0; k < nbins; ++k) {
+        const double lower = -(mel_f[m] - fft_f[k]) / (mel_f[m + 1] - mel_f[m]);
+        const double upper = (mel_f[m + 2] - fft_f[k]) / (mel_f[m + 2] - mel_f[m + 1]);
+        const float w = (float)std::max(0.0, std::min(lower, upper));
+        row[k] = (float)((double)w * enorm);
+        if (row[k] != 0.f) { if (first < 0) first = k; last = k; }
+      }
+      off[m] = (int32_t)wpack.size();
+      lo[m] = first < 0 ? 0 : first;
+      if (first >= 0) wpack.insert(wpack.end(), row.begin() + first, row.begin() + last + 1);
+    }
+    off[n_mels] = (int32_t)wpack.size();
+    std::vector<char> img(b_off + b_lo + sizeof(float) * wpack.size());
+    memcpy(img.data(), off.data(), b_off);
+    memcpy(img.data() + b_off, lo.data(), b_lo);
+    if (!wpack.empty()) memcpy(img.data() + b_off + b_lo, wpack.data(), sizeof(float) * wpack.size());
+    return img;
+  }, &p);
+  if (e != cudaSuccess) return e;
+  out->off = reinterpret_cast<const int32_t*>(p);
+  out->lo = reinterpret_cast<const int32_t*>(p + b_off);
+  out->w = reinterpret_cast<const float*>(p + b_off + b_lo);
+  return cudaSuccess;
+}
+
+cudaError_t launch_spectrogram(SpecMode mode, const float* samples, int rows, int N, int hop, int n_fft,
+                               const FftTables& fft, const MelBank& bank, int n_mels, float* out, cudaStream_t st) {
+  const int F = 1 + N / hop;
+  const MelSpecArgs t{fft, bank, n_mels};
+#define SPEC_LAUNCH(NF, MODE)                                                                                    \
+  mel_spec_kernel<NF, MODE><<<dim3((F + MelGeom<NF>::FPC - 1) / MelGeom<NF>::FPC, rows), THREADS, 0, st>>>(      \
+      samples, N, F, hop, t, out)
+  if (mode == SpecMode::ONSET_DB) {
+    if (n_fft != ONSET_NFFT || n_mels != ONSET_NMELS) return cudaErrorInvalidValue;
+    SPEC_LAUNCH(ONSET_NFFT, SpecMode::ONSET_DB);
+  } else {
+    switch (n_fft) {
+#define MEL_CASE(NF) case NF: SPEC_LAUNCH(NF, SpecMode::MEL_MAG); break;
+      MEL_CASE(32) MEL_CASE(64) MEL_CASE(128) MEL_CASE(256) MEL_CASE(512) MEL_CASE(1024) MEL_CASE(2048) MEL_CASE(4096)
+#undef MEL_CASE
+      default: return cudaErrorInvalidValue;
+    }
+  }
+#undef SPEC_LAUNCH
+  count_launch();
+  return cudaGetLastError();
+}
 
 MelLossPlan mel_loss_plan(int B, int C, int N, int sr, const vnb_mel_scale* scales, int n_scales) {
   MelLossPlan p;
@@ -184,11 +271,12 @@ MelLossPlan mel_loss_plan(int B, int C, int N, int sr, const vnb_mel_scale* scal
     spec = std::max(spec, (size_t)B * (size_t)s.elems * sizeof(float));
   }
   // one X and one Y buffer, reused scale after scale (the stream orders the reuse)
-  p.x_spec = 0;
-  p.y_spec = align256(spec);
-  p.partials = p.y_spec + align256(spec);
-  p.items = p.partials + align256(partials * sizeof(double2));
-  p.total = p.items + align256((size_t)B * n_scales * sizeof(double2));
+  size_t o = 0;
+  p.x_spec = carve(o, spec);
+  p.y_spec = carve(o, spec);
+  p.partials = carve(o, partials * sizeof(double2));
+  p.items = carve(o, (size_t)B * n_scales * sizeof(double2));
+  p.total = o;
   return p;
 }
 
@@ -197,7 +285,7 @@ cudaError_t launch_mel_spectrogram(const float* samples, int rows, int N, int sr
   MelSpecArgs t;
   cudaError_t e = spec_args(sr, s, &t);
   if (e != cudaSuccess) return e;
-  return spec_launch(samples, rows, N, 1 + N / s.hop, s.hop, t, out, s.n_fft, st);
+  return launch_spectrogram(SpecMode::MEL_MAG, samples, rows, N, s.hop, s.n_fft, t.fft, t.bank, t.n_mels, out, st);
 }
 
 cudaError_t launch_mel_loss(const float* x, const float* y, const MelLossPlan& p, double clamp_eps, double pow,
@@ -216,8 +304,10 @@ cudaError_t launch_mel_loss(const float* x, const float* y, const MelLossPlan& p
     MelSpecArgs t;
     cudaError_t e = spec_args(p.sr, sc, &t);
     if (e != cudaSuccess) return e;
-    if ((e = spec_launch(x, rows, p.N, s.F, s.hop, t, X, s.n_fft, st)) != cudaSuccess) return e;
-    if ((e = spec_launch(y, rows, p.N, s.F, s.hop, t, Y, s.n_fft, st)) != cudaSuccess) return e;
+    if ((e = launch_spectrogram(SpecMode::MEL_MAG, x, rows, p.N, s.hop, s.n_fft, t.fft, t.bank, t.n_mels, X, st)))
+      return e;
+    if ((e = launch_spectrogram(SpecMode::MEL_MAG, y, rows, p.N, s.hop, s.n_fft, t.fft, t.bank, t.n_mels, Y, st)))
+      return e;
     mel_diff_kernel<<<dim3(s.chunks, p.B), THREADS, 0, st>>>(X, Y, s.elems, s.chunks, clamp_eps, pow, partial + s.partial);
     count_launch();
     a.chunks[i] = s.chunks;

@@ -15,12 +15,7 @@
 // oracle/pitch_oracle.py restates the same steps in float64 numpy.
 #include <algorithm>
 #include <cmath>
-#include <cstring>
-#include <map>
-#include <mutex>
 #include <numeric>
-#include <tuple>
-#include <vector>
 
 #include "kernels.h"
 
@@ -274,15 +269,6 @@ __global__ void time_steps_kernel(float rate, long long n, float* __restrict__ o
 
 int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
-struct BasisSet {
-  double* fwd = nullptr;
-  double* inv = nullptr;
-};
-std::mutex g_basis_mu;
-std::map<std::pair<int, int>, BasisSet> g_basis;  // (device, n_fft)
-
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
-
 int grid_for(long long n, int threads) { return (int)std::min<long long>((n + threads - 1) / threads, 65535); }
 }  // namespace
 
@@ -319,30 +305,29 @@ PitchLayout pitch_layout(const PitchPlan& p) {
   const size_t R = (size_t)p.rows, z = sizeof(double);
   PitchLayout l;
   size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += align256(bytes); return at; };
-  l.spec = take(R * p.F * p.nb * 2 * z);                            // spectrum, then (|X|, angle)
-  l.stretched = p.stretch ? take(R * p.F2 * p.nb * 2 * z) : l.spec;  // stretched spectrum
-  l.chunk = p.stretch ? take(R * p.nchunks * p.nb * z) : 0;          // chunk sums
-  l.frames = take(R * p.F2 * p.n_fft * z);                          // inverse DFT frames
-  l.y = take(R * p.L * z);                                          // overlap-added signal
+  l.spec = carve(o, R * p.F * p.nb * 2 * z);                            // spectrum, then (|X|, angle)
+  l.stretched = p.stretch ? carve(o, R * p.F2 * p.nb * 2 * z) : l.spec;  // stretched spectrum
+  l.chunk = p.stretch ? carve(o, R * p.nchunks * p.nb * z) : 0;          // chunk sums
+  l.frames = carve(o, R * p.F2 * p.n_fft * z);                          // inverse DFT frames
+  l.y = carve(o, R * p.L * z);                                          // overlap-added signal
   l.total = o;
   return l;
 }
 
 size_t pitch_workspace_bytes(const PitchPlan& p) { return pitch_layout(p).total; }
 
+// one table: the forward basis, then the inverse at a 256-byte aligned offset
 cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  std::lock_guard<std::mutex> lock(g_basis_mu);
-  auto key = std::make_pair(dev, n_fft);
-  auto it = g_basis.find(key);
-  if (it == g_basis.end()) {
-    const int nb = n_fft / 2 + 1;
-    const int fk = round_up(n_fft, BK), fn = round_up(2 * nb, BN);  // forward: (n_fft x 2 nb), re/im interleaved
-    const int ik = round_up(2 * nb, BK), in = round_up(n_fft, BN);  // inverse: (2 nb x n_fft)
-    std::vector<double> f((size_t)fk * fn, 0.0), v((size_t)ik * in, 0.0);
+  const int nb = n_fft / 2 + 1;
+  const int fk = round_up(n_fft, BK), fn = round_up(2 * nb, BN);  // forward: (n_fft x 2 nb), re/im interleaved
+  const int ik = round_up(2 * nb, BK), in = round_up(n_fft, BN);  // inverse: (2 nb x n_fft)
+  size_t o = 0;
+  const size_t f_at = carve(o, (size_t)fk * fn * sizeof(double)), v_at = carve(o, (size_t)ik * in * sizeof(double));
+  const char* p = nullptr;
+  cudaError_t e = device_table({TABLE_PITCH_BASIS, (double)n_fft}, [&] {
+    std::vector<char> img(o);  // zeroed: the tile padding stays 0
+    double* f = reinterpret_cast<double*>(img.data() + f_at);
+    double* v = reinterpret_cast<double*>(img.data() + v_at);
     for (int n = 0; n < n_fft; ++n)
       for (int k = 0; k < nb; ++k) {
         const double a = 2.0 * M_PI * (double)(((long long)k * n) % n_fft) / n_fft;  // argument reduced exactly
@@ -354,18 +339,11 @@ cudaError_t pitch_basis(int n_fft, const double** fwd, const double** inv) {
         v[(size_t)(2 * k) * in + n] = (edge ? 1.0 : 2.0) * co / n_fft;
         v[(size_t)(2 * k + 1) * in + n] = edge ? 0.0 : -2.0 * si / n_fft;
       }
-    BasisSet s;
-    e = cudaMalloc(&s.fwd, f.size() * sizeof(double));
-    if (e != cudaSuccess) return e;
-    e = cudaMalloc(&s.inv, v.size() * sizeof(double));
-    if (e != cudaSuccess) { cudaFree(s.fwd); return e; }
-    e = cudaMemcpy(s.fwd, f.data(), f.size() * sizeof(double), cudaMemcpyHostToDevice);  // once per (device, n_fft)
-    if (e == cudaSuccess) e = cudaMemcpy(s.inv, v.data(), v.size() * sizeof(double), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { cudaFree(s.fwd); cudaFree(s.inv); return e; }
-    it = g_basis.emplace(key, s).first;
-  }
-  *fwd = it->second.fwd;
-  *inv = it->second.inv;
+    return img;
+  }, &p);
+  if (e != cudaSuccess) return e;
+  *fwd = reinterpret_cast<const double*>(p + f_at);
+  *inv = reinterpret_cast<const double*>(p + v_at);
   return cudaSuccess;
 }
 

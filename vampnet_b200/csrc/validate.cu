@@ -208,12 +208,21 @@ __global__ void xent_final_kernel(const XentItem* __restrict__ items, const doub
       }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+// the workspace: the rows' records, then the items'
+struct XentLayout {
+  size_t rows, items, total;
+};
+XentLayout xent_layout(long long B, long long S) {
+  XentLayout l;
+  size_t o = 0;
+  l.rows = carve(o, (size_t)(B * S) * sizeof(XentRow));
+  l.items = carve(o, (size_t)B * sizeof(XentItem));
+  l.total = o;
+  return l;
+}
 }  // namespace
 
-size_t xent_workspace_bytes(long long B, long long S) {
-  return align256((size_t)(B * S) * sizeof(XentRow)) + (size_t)B * sizeof(XentItem);
-}
+size_t xent_workspace_bytes(long long B, long long S) { return xent_layout(B, S).total; }
 
 cudaError_t launch_xent_rows(const float* logits, const int64_t* z, int B, int C, int T, int ncc, int V, XentRow* rows,
                              cudaStream_t st) {
@@ -228,8 +237,9 @@ cudaError_t launch_xent_metrics(const float* logits, const int64_t* z, const int
                                 int C, int T, int ncc, int V, double eps, void* workspace, float* out,
                                 int32_t* ambiguous, cudaStream_t st) {
   const long long S = (long long)T * (C - ncc);
-  XentRow* rows = static_cast<XentRow*>(workspace);
-  XentItem* items = reinterpret_cast<XentItem*>(static_cast<char*>(workspace) + align256((size_t)(B * S) * sizeof(XentRow)));
+  const XentLayout l = xent_layout(B, S);
+  XentRow* rows = reinterpret_cast<XentRow*>(static_cast<char*>(workspace) + l.rows);
+  XentItem* items = reinterpret_cast<XentItem*>(static_cast<char*>(workspace) + l.items);
   cudaError_t e = launch_xent_rows(logits, z, B, C, T, ncc, V, rows, st);
   if (e != cudaSuccess) return e;
   xent_items_kernel<<<B, ITEM_THREADS, 0, st>>>(rows, mask, S, C, T, ncc, items);

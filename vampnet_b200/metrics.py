@@ -38,14 +38,12 @@ def xent_metrics(logits: torch.Tensor, z: torch.Tensor, mask: torch.Tensor, r: t
     mask = mask.to(dev, torch.int64).contiguous()
     r = r.to(dev, torch.float64).contiguous()
     L = _lib.lib()
-    need = C.c_uint64()
-    _lib.check(L.vnb_xent_metrics_workspace_bytes(B, T * (C_ - ncc), C.byref(need)))
-    ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+    ws, ws_bytes = _lib.workspace(dev, L.vnb_xent_metrics_workspace_bytes, B, T * (C_ - ncc))
     out = torch.empty(len(KEYS), dtype=torch.float32, device=dev)
     amb = torch.empty(len(KEYS), dtype=torch.int32, device=dev) if return_ambiguous else None
     with torch.cuda.device(dev):
         _lib.check(L.vnb_xent_metrics(_lib.ptr(logits), _lib.ptr(z), _lib.ptr(mask), _lib.ptr(r), B, C_, T, ncc, V,
-                                      float(label_smoothing), _lib.ptr(ws), need.value, _lib.ptr(out),
+                                      float(label_smoothing), _lib.ptr(ws), ws_bytes, _lib.ptr(out),
                                       _lib.ptr(amb) if amb is not None else None, _lib.stream_ptr(dev)))
     return (out, amb) if return_ambiguous else out
 
@@ -141,15 +139,13 @@ class MelSpectrogramLoss(torch.nn.Module):
         scales = (_lib.MelScale * n)(*[_scale(sr, m, lo, hi, w, w // 4) for m, lo, hi, w in
                                        zip(self.n_mels, self.mel_fmin, self.mel_fmax, self.window_lengths)])
         L = _lib.lib()
-        need = C.c_uint64()
-        _lib.check(L.vnb_mel_workspace_bytes(B, Ch, N, sr, scales, n, C.byref(need)))
+        ws, ws_bytes = _lib.workspace(dev, L.vnb_mel_workspace_bytes, B, Ch, N, sr, scales, n)
         loss = torch.empty((), dtype=torch.float32, device=dev)
         items = torch.empty(B, dtype=torch.float32, device=dev) if per_item else None
         with torch.cuda.device(dev):
-            ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
             _lib.check(L.vnb_mel_loss(_lib.ptr(xs), _lib.ptr(ys), B, Ch, N, sr, scales, n, float(self.clamp_eps),
                                       float(self.pow), float(self.log_weight), float(self.mag_weight), _lib.ptr(ws),
-                                      need.value, _lib.ptr(loss), _lib.ptr(items), _lib.stream_ptr(dev)))
+                                      ws_bytes, _lib.ptr(loss), _lib.ptr(items), _lib.stream_ptr(dev)))
         return (items if per_item else loss).to(home)
 
     def forward(self, x, y) -> torch.Tensor:

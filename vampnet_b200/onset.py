@@ -23,33 +23,37 @@ def n_frames(n_samples: int, hop_length: int) -> int:
     return 1 + n_samples // hop_length
 
 
-def onset_detect(samples: torch.Tensor, sample_rate: int, hop_length: int, backtrack: bool = True) -> Onsets:
-    """Onsets of every row of ``samples`` ((N,) or (B, N) float32 on a CUDA device), each row analysed on its own.
-    With ``backtrack`` each onset moves to the preceding local minimum of the envelope, as librosa's does."""
+def as_rows(samples: torch.Tensor, who: str) -> torch.Tensor:
+    """``samples`` ((N,) or (B, N) float32 on a CUDA device) as a contiguous (B, N) tensor; RuntimeError otherwise."""
     if not torch.is_tensor(samples) or samples.dtype != torch.float32:
-        raise RuntimeError(f"onset_detect: samples must be a float32 tensor, got {getattr(samples, 'dtype', type(samples))}")
+        raise RuntimeError(f"{who}: samples must be a float32 tensor, got {getattr(samples, 'dtype', type(samples))}")
     if samples.device.type != "cuda":
-        raise RuntimeError(f"onset_detect: samples must be on a CUDA device, got {samples.device}")
+        raise RuntimeError(f"{who}: samples must be on a CUDA device, got {samples.device}")
     if samples.ndim == 1:
         samples = samples[None]
     if samples.ndim != 2:
-        raise RuntimeError(f"onset_detect: samples must be (N,) or (B, N), got {tuple(samples.shape)}")
-    samples = samples.contiguous()
+        raise RuntimeError(f"{who}: samples must be (N,) or (B, N), got {tuple(samples.shape)}")
+    return samples.contiguous()
+
+
+def onset_detect(samples: torch.Tensor, sample_rate: int, hop_length: int, backtrack: bool = True) -> Onsets:
+    """Onsets of every row of ``samples`` ((N,) or (B, N) float32 on a CUDA device), each row analysed on its own.
+    With ``backtrack`` each onset moves to the preceding local minimum of the envelope, as librosa's does."""
+    samples = as_rows(samples, "onset_detect")
     B, N = samples.shape
     L = _lib.lib()
     hop = int(hop_length)
     F = n_frames(N, hop) if hop > 0 else 1
     dev = samples.device
-    ws_bytes = _lib.C.c_uint64(0)
-    if B > 0 and N > 0 and hop > 0:
-        _lib.check(L.vnb_onset_workspace_bytes(B, N, hop, _lib.C.byref(ws_bytes)))
+    # out-of-range shapes go straight to vnb_onset_detect, which names them
+    workspace, ws_bytes = (_lib.workspace(dev, L.vnb_onset_workspace_bytes, B, N, hop) if B > 0 and N > 0 and hop > 0
+                           else (None, 0))
     with torch.cuda.device(dev):
-        workspace = torch.empty(max(int(ws_bytes.value), 1), dtype=torch.uint8, device=dev)
         frames = torch.empty(max(B, 1), F, dtype=torch.int32, device=dev)
         counts = torch.empty(max(B, 1), dtype=torch.int32, device=dev)
         envelope = torch.empty(max(B, 1), F, dtype=torch.float32, device=dev)
         _lib.check(L.vnb_onset_detect(_lib.ptr(samples), B, N, int(sample_rate), hop, int(bool(backtrack)),
-                                      _lib.ptr(workspace), ws_bytes.value, _lib.ptr(envelope), _lib.ptr(frames),
+                                      _lib.ptr(workspace), ws_bytes, _lib.ptr(envelope), _lib.ptr(frames),
                                       _lib.ptr(counts), _lib.stream_ptr(dev)))
     return Onsets(frames, counts, envelope)
 

@@ -44,14 +44,12 @@ def pitch_shift(input: torch.Tensor, shift, sample_rate: int, bins_per_octave: i
     n_fft, hop, new_freq, rate = shift_params(shift, sample_rate, bins_per_octave, n_fft, hop_length)
     x = input.reshape(B * Ch, N).contiguous()
     L = _lib.lib()
-    ws_bytes = _lib.C.c_uint64(0)
     args = (B * Ch, N, int(sample_rate), new_freq, n_fft, hop, rate)
-    _lib.check(L.vnb_pitch_workspace_bytes(*args, _lib.C.byref(ws_bytes)))
     dev = input.device
+    workspace, ws_bytes = _lib.workspace(dev, L.vnb_pitch_workspace_bytes, *args)
     with torch.cuda.device(dev):
-        workspace = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
         out = torch.empty_like(x)
-        _lib.check(L.vnb_pitch_shift(_lib.ptr(x), *args, _lib.ptr(workspace), ws_bytes.value, _lib.ptr(out),
+        _lib.check(L.vnb_pitch_shift(_lib.ptr(x), *args, _lib.ptr(workspace), ws_bytes, _lib.ptr(out),
                                      _lib.stream_ptr(dev)))
     return out.reshape(B, Ch, N)
 
