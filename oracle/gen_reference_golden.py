@@ -2,8 +2,8 @@
 
     VAMPNET_REFERENCE_ROOT=<checkout of the original vampnet> python -m oracle.gen_reference_golden
 
-Writes tests/golden/reference_{mask,vampnet,interface}.npz.  The tests (test_mask_cpu, test_oracle_vs_reference,
-test_interface_vs_reference) recompute their side with the same seeds and compare with these arrays, so they need
+Writes tests/golden/reference_{mask,vampnet,vampnet_configs,interface}.npz.  The tests (test_mask_cpu,
+test_oracle_vs_reference, test_oracle_configs_vs_reference, test_interface_vs_reference) recompute their side with the same seeds and compare with these arrays, so they need
 no checkout of the original.  Kept small: token ids and masks as int16, and where a test compared large fp32 tensors
 a fixed seeded sample of their entries (``sample_idx``).
 """
@@ -90,29 +90,38 @@ CFGS = {
 GEN_KWS = [dict(sample_cutoff=-1.0, mask_temperature=0.0), dict(), dict(temperature=1.3, top_p=0.8),
            dict(sample_cutoff=0.4)]
 GEN_STEPS = (1, 2, 7)
+# off the shipped geometry (vocab_size != 1024, a single predicted codebook, an odd number of them): configurations A and
+# C of tests/test_gpu_model_configs.py, at fewer layers
+CONFIG_CFGS = {
+    "v256_cp1": dict(n_heads=8, n_layers=1, n_codebooks=1, n_conditioning_codebooks=0, embedding_dim=512,
+                     vocab_size=256),
+    "v768_cp7": dict(n_heads=16, n_layers=1, n_codebooks=9, n_conditioning_codebooks=2, embedding_dim=1024,
+                     vocab_size=768),
+}
 
 
-def vampnet_case(tag, lora):
+def vampnet_case(tag, lora, cfgs=CFGS):
     """Inputs of one forward / generate case (everything seeded)."""
-    cfgd = CFGS[tag]
+    cfgd = cfgs[tag]
     cfg = vo.OracleConfig(**cfgd)
+    V = cfg.vocab_size
     sd = vo.make_state_dict(cfg, seed=7, lora=lora)
-    cb = vo.make_codebooks(cfg.n_codebooks, seed=2)
+    cb = vo.make_codebooks(cfg.n_codebooks, vocab_size=V, seed=2)
     g = torch.Generator().manual_seed(3)
-    z = torch.randint(0, 1024, (3, cfg.n_codebooks, 31), generator=g)
+    z = torch.randint(0, V, (3, cfg.n_codebooks, 31), generator=g)
     zm = z.clone()
-    zm[:, cfg.n_conditioning_codebooks:, ::2] = 1024
+    zm[:, cfg.n_conditioning_codebooks:, ::2] = cfg.mask_token
     mask = torch.ones_like(z)
     mask[:, :, ::5] = 0
     return cfgd, cfg, sd, cb, z, zm, mask
 
 
-def gen_vampnet(tr):
+def gen_vampnet(tr, cfgs=CFGS, loras=(False, True), extras=True):
     out = {}
-    for tag in CFGS:
-        for lora in (False, True):
+    for tag in cfgs:
+        for lora in loras:
             key = f"{tag}_lora{int(lora)}"
-            cfgd, cfg, sd, cb, z, zm, mask = vampnet_case(tag, lora)
+            cfgd, cfg, sd, cb, z, zm, mask = vampnet_case(tag, lora, cfgs)
             ref = tr.VampNet(flash_attn=False, **cfgd)
             res = ref.load_state_dict(sd, strict=False)
             assert not res.unexpected_keys
@@ -133,6 +142,8 @@ def gen_vampnet(tr):
                     zr = ref.generate(codec, start_tokens=z.clone(), mask=mask.clone(), _sampling_steps=steps, seed=9,
                                       return_signal=False, **kw)
                     out[f"{key}_gen{ki}_s{steps}"] = i16(zr)
+    if not extras:
+        return out
     # typical_filter: the reference discards its result (transformer.py:989-993)
     logits = torch.randn(2, 9, 1024, generator=torch.Generator().manual_seed(0))
     torch.manual_seed(1)
@@ -159,6 +170,11 @@ def gen_vampnet(tr):
                           seed=1, return_signal=False)
         out[name] = i16(zr)
     return out
+
+
+def gen_vampnet_configs(tr):
+    """The reference at CONFIG_CFGS: forward and generate with a vocabulary, and so a mask token, other than 1024."""
+    return gen_vampnet(tr, CONFIG_CFGS, loras=(False,), extras=False)
 
 
 # ------------------------------------------------------------------------------------------------ Interface
@@ -248,11 +264,12 @@ def main():
     try:
         np.savez_compressed(os.path.join(GOLDEN, "reference_mask.npz"), **gen_mask(rm))
         np.savez_compressed(os.path.join(GOLDEN, "reference_vampnet.npz"), **gen_vampnet(tr))
+        np.savez_compressed(os.path.join(GOLDEN, "reference_vampnet_configs.npz"), **gen_vampnet_configs(tr))
         np.savez_compressed(os.path.join(GOLDEN, "reference_interface.npz"),
                             **gen_interface(ref_shims.load_reference_interface()))
     finally:
         ref_shims.uninstall()
-    for n in ("mask", "vampnet", "interface"):
+    for n in ("mask", "vampnet", "vampnet_configs", "interface"):
         p = os.path.join(GOLDEN, f"reference_{n}.npz")
         print(p, os.path.getsize(p), "bytes")
 

@@ -248,28 +248,28 @@ SAMPLE_GRID = [(t, s, st) for t in (0.05, 0.7, 1.0, 3.0) for s in (0, 1) for st 
 SEED = (2024, 77)
 
 
-def check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, grid):
+def check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, grid, V=GB.V):
     """Runs the sampling epilogue for every (temperature, do_sample, step) of `grid` and checks every record against
     tests/gemm_sample_ref.py, with the logits L from BIAS_F32 on the same operands and row scale (the epilogue
     computes each logit with the same two roundings):  max exact; arg-max exact (lowest index on ties); sum within
     1e-5 relative of float64 (ex2.approx and a 128-term fp32 sum); candidate exact unless its crossing lies within
     1e-5 * sum of the target; the record's logit == L[candidate]; greedy: candidate == arg-max; known positions and
-    everything past the last row keep the sentinel."""
+    everything past the last row keep the sentinel.  V is the vocabulary size (and the mask token)."""
     M, K = A.shape
-    Cp, nt = C - ncc, GB.V // 128
-    N = Cp * GB.V
+    Cp, nt = C - ncc, V // 128
+    N = Cp * V
     Bn = M // T
     G = 64
     logits = GB.sentinel((M, N), torch.float32)
     GB.gemm_fused(L.EPI_BIAS_F32, A, W, logits, bias=bias, ss_in=ss, inv_d=inv_d)
-    masked = (zcur[:, ncc:] == GB.V)                                   # (M, Cp)
+    masked = (zcur[:, ncc:] == V)                                      # (M, Cp)
     rows_m, cps_m = masked.nonzero(as_tuple=True)
     ambiguous = compared = 0
     for temperature, do_sample, step in grid:
         rec = GB.sentinel((M * Cp * nt + G, 4), torch.float32)
-        GB.gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, SEED, rec)
+        GB.gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, SEED, rec, V=V)
         torch.cuda.synchronize()
-        what = f"T={temperature} sample={do_sample} step={step}"
+        what = f"V={V} T={temperature} sample={do_sample} step={step}"
         assert_untouched(rec[M * Cp * nt:], what + ": records past the last row")
         recs = rec[: M * Cp * nt].view(M, Cp, nt, 4)
         assert bool(GB.untouched(recs[~masked]).all()), what + ": a known position's record was written"
@@ -279,7 +279,7 @@ def check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, grid):
         inv_t = SR.inv_temperature(temperature)
         for i0 in range(0, rows_m.numel(), 65536):
             r, cp = rows_m[i0:i0 + 65536], cps_m[i0:i0 + 65536]
-            x = logits[r[:, None], cp[:, None] * GB.V + torch.arange(GB.V, device="cuda")].reshape(-1, 128)
+            x = logits[r[:, None], cp[:, None] * V + torch.arange(V, device="cuda")].reshape(-1, 128)
             u2 = None
             if do_sample:
                 u2 = u2_all[r // T, (r % T) * Cp + cp].repeat_interleave(nt)
@@ -303,14 +303,14 @@ def check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, grid):
     assert ambiguous <= compared // 1000 + 1, f"{ambiguous} of {compared} draws too close to call"
 
 
-def sample_case(M, T, C, ncc, d=1280, seed=0):
-    N = (C - ncc) * GB.V
+def sample_case(M, T, C, ncc, d=1280, seed=0, V=GB.V):
+    N = (C - ncc) * V
     A, W, g = GB.operands(M, N, d, seed=seed)
     bias = torch.randn(N, generator=g)
     W = W.cpu()
-    GB.tie_columns(W, bias, g)
+    GB.tie_columns(W, bias, g, V=V)
     ss, inv_d, _ = GB.row_stats(M, d, d // 128, g)
-    return A, W.cuda(), bias.cuda(), ss, inv_d, GB.sample_inputs(M, C, ncc, g)
+    return A, W.cuda(), bias.cuda(), ss, inv_d, GB.sample_inputs(M, C, ncc, g, V=V)
 
 
 @pytest.mark.parametrize("C,ncc", [(4, 0), (14, 4)], ids=["coarse", "c2f"])
@@ -325,6 +325,20 @@ def test_sample_records_benchmark_size(L, pair):
     B, T, C, ncc = 32, 768, 14, 4
     A, W, bias, ss, inv_d, zcur = sample_case(B * T, T, C, ncc, seed=19)
     check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, [(0.7, 1, 11)])
+
+
+VOCAB_GRID = [(0.05, 1, 11), (0.7, 1, 0), (1.0, 0, 0), (3.0, 1, 11)]
+
+
+@pytest.mark.parametrize("C,ncc", [(1, 0), (4, 1), (9, 2)], ids=["cp1", "cp3", "cp7"])
+@pytest.mark.parametrize("V", [256, 512, 768])
+def test_sample_records_vocab_sizes(L, pair, V, C, ncc):
+    """Every vocabulary size the library accepts below 1024 (2, 4 and 6 strips per codebook; the record index and the
+    mask token both depend on it) with one, three and seven predicted codebooks, at d = 512 and ragged M = 3 x 150:
+    each record must equal the float64 reference and nothing outside the masked positions' records may be written."""
+    B, T = 3, 150
+    A, W, bias, ss, inv_d, zcur = sample_case(B * T, T, C, ncc, d=512, seed=20 + V + C, V=V)
+    check_sample_records(L, A, W, bias, ss, inv_d, zcur, T, C, ncc, VOCAB_GRID, V=V)
 
 
 # ------------------------------------------------------------------------------------------ determinism

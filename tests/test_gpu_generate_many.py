@@ -38,10 +38,10 @@ def mix(cfg, seed):
     sample cutoffs 1, 0.5 and -1 (true greedy), 3-D, 2-D and absent masks, two T buckets, a bucket with a different
     step count, and a top-p bucket whose calls use different top_p."""
     g = torch.Generator().manual_seed(seed)
-    C = cfg["n_codebooks"]
+    C, V = cfg["n_codebooks"], cfg.get("vocab_size", 1024)
 
     def z(B, T):
-        return torch.randint(0, 1024, (B, C, T), generator=g).cuda()
+        return torch.randint(0, V, (B, C, T), generator=g).cuda()
 
     def m3(B, T):
         return (torch.rand(B, C, T, generator=g) < 0.6).long().cuda()

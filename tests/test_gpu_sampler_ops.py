@@ -131,7 +131,7 @@ DRAW = [(0.05, 0.0, 1), (1.0, 10.5, 1), (3.0, 4.0, 1), (-1.0, 10.5, 1), (0.7, 10
 
 @pytest.mark.parametrize("temperature,temp_eff,do_sample", DRAW,
                          ids=["T0.05_te0", "T1_te10.5", "T3_te4", "Tneg_te10.5", "greedy"])
-@pytest.mark.parametrize("V", [128, 256, 768, 1024])
+@pytest.mark.parametrize("V", [128, 256, 512, 768, 1024])
 @pytest.mark.parametrize("C,ncc", [(4, 0), (14, 4)], ids=["coarse", "c2f"])
 @pytest.mark.parametrize("path", [0, 1], ids=["rows", "topp"])
 def test_materialised_draw(path, C, ncc, V, temperature, temp_eff, do_sample):
@@ -245,21 +245,32 @@ def test_combine_real_records(C, ncc, temperature, do_sample, step):
     gemm_sample_ref.combine of the float64 records of the same logits, confidences are within the bound against
     float64 softmax, and path 0 on the materialised logits gives the same tokens except on ambiguous rows.  Records of
     known positions are never written by the epilogue (they hold a NaN sentinel) and must not be read."""
-    B, T, d, V = 3, 150, 1280, GB.V
+    check_combine_real_records(C, ncc, temperature, do_sample, step, GB.V)
+
+
+@pytest.mark.parametrize("C,ncc", [(4, 0), (14, 4), (1, 0)], ids=["coarse", "c2f", "cp1"])
+@pytest.mark.parametrize("temperature,do_sample,step", [(0.7, 1, 11), (1.0, 0, 0), (3.0, 1, 2)])
+def test_combine_real_records_v512(C, ncc, temperature, do_sample, step):
+    """test_combine_real_records at a 512-entry vocabulary: four records per position."""
+    check_combine_real_records(C, ncc, temperature, do_sample, step, 512)
+
+
+def check_combine_real_records(C, ncc, temperature, do_sample, step, V):
+    B, T, d = 3, 150, 1280
     Cp = C - ncc
     M, N, S, nt = B * T, Cp * V, T * Cp, V // 128
-    A, W, gg = GB.operands(M, N, d, seed=31 + C)
+    A, W, gg = GB.operands(M, N, d, seed=31 + C + (V != GB.V) * V)
     bias = torch.randn(N, generator=gg)
     W = W.cpu()
-    GB.tie_columns(W, bias, gg)
+    GB.tie_columns(W, bias, gg, V=V)
     W, bias = W.cuda(), bias.cuda()
     ss, inv_d, _ = GB.row_stats(M, d, d // 128, gg)
-    zcur = GB.sample_inputs(M, C, ncc, gg)
+    zcur = GB.sample_inputs(M, C, ncc, gg, V=V)
     logits = GB.sentinel((M, N), torch.float32)
     GB.gemm_fused(GB.lib().EPI_BIAS_F32, A, W, logits, bias=bias, ss_in=ss, inv_d=inv_d)
     logits = logits.view(M * Cp, V)
     rec = GB.sentinel((M * Cp * nt, 4), torch.float32)
-    GB.gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, SEED, rec)
+    GB.gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, SEED, rec, V=V)
     torch.cuda.synchronize()
     z3 = zcur.view(B, T, C)
     grp = Group(rows=B, temperature=temperature, gamma=0.45, temp_eff=10.5 * (1 - step / 12), do_sample=do_sample,

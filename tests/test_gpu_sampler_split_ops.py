@@ -47,17 +47,27 @@ def row_ranges(groups):
 
 @pytest.mark.parametrize("C,ncc", [(4, 0), (14, 4)], ids=["coarse", "c2f"])
 def test_split_epilogue_equals_bias_f32_and_sample_records(C, ncc):
+    check_split_epilogue(C, ncc, GB.V)
+
+
+@pytest.mark.parametrize("V,C,ncc", [(256, 1, 0), (256, 3, 1), (768, 9, 2)], ids=["v256_cp1", "v256_cp2", "v768_cp7"])
+def test_split_epilogue_vocab_sizes(V, C, ncc):
+    """The split epilogue at 2 and 6 strips per codebook, with one, two and seven predicted codebooks."""
+    check_split_epilogue(C, ncc, V)
+
+
+def check_split_epilogue(C, ncc, V):
     L = GB.lib()
-    d, V = 512, GB.V
+    d = 512
     Cp = C - ncc
     M, N, nt = B * T, Cp * V, V // 128
-    A, W, gg = GB.operands(M, N, d, seed=50 + C)
+    A, W, gg = GB.operands(M, N, d, seed=50 + C + (V != GB.V) * V)
     bias = torch.randn(N, generator=gg)
     W = W.cpu()
-    GB.tie_columns(W, bias, gg)
+    GB.tie_columns(W, bias, gg, V=V)
     W, bias = W.cuda(), bias.cuda()
     ss, inv_d, _ = GB.row_stats(M, d, d // 128, gg)
-    zcur = GB.sample_inputs(M, C, ncc, gg)
+    zcur = GB.sample_inputs(M, C, ncc, gg, V=V)
     # the materialised logits and, per plain group, the records of the group launched alone
     want_logits = GB.sentinel((M, N), torch.float32)
     GB.gemm_fused(L.EPI_BIAS_F32, A, W, want_logits, bias=bias, ss_in=ss, inv_d=inv_d)
@@ -66,7 +76,8 @@ def test_split_epilogue_equals_bias_f32_and_sample_records(C, ncc):
         if not top_p_on(g.top_p):
             rows = slice(b0 * T, b1 * T)
             GB.gemm_sample(A[rows], W, bias, ss[:, rows].contiguous(), inv_d, zcur[rows].contiguous(), T, C, ncc,
-                           g.temperature, g.do_sample, g.step, g.seed, want_rec[b0 * T * Cp * nt:b1 * T * Cp * nt])
+                           g.temperature, g.do_sample, g.step, g.seed, want_rec[b0 * T * Cp * nt:b1 * T * Cp * nt],
+                           V=V)
     logits = GB.sentinel((M, N), torch.float32)
     rec = GB.sentinel((M * Cp * nt, 4), torch.float32)
     L.check(L.lib().vnb_dbg_gemm_sample_split(L.ptr(A), L.ptr(W), L.ptr(bias), M, N, d, L.ptr(ss), ss.shape[0], inv_d,

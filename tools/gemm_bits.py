@@ -1,6 +1,7 @@
 """Bit-level record of the GEMM family's fused epilogues (vnb_dbg_gemm_fused, vnb_dbg_gemm_sample) on seeded inputs:
 
     python tools/gemm_bits.py --write tests/golden/gemm_bits.npz
+    python tools/gemm_bits.py --add-to tests/golden/gemm_bits.npz --write <new record>   # new cases only
 
 Every case builds its operands on the CPU from a fixed seed, runs the library on cuda:0 and stores the SHA-256 of
 all of its outputs (bit patterns, in a fixed order) plus a fixed seeded sample of its first output's values (for
@@ -10,7 +11,8 @@ so a rewrite of the epilogues that alters any float operation or its order is ca
 The cases cover every fused variant the forward launches, at d_model 256 (ss_parts 2) and 1280 (ss_parts 10), with
 ragged M: the row-scaled consumers (BF16, QKV with vT and batch boundaries inside a tile, GEGLU, the classifier's
 BIAS_F32), the producers (RESID with its bf16 copy and two sum-of-squares partials per tile, the embedding projection's
-BIAS_F32 with one partial per tile) and the sampling epilogue for both codebook layouts (C, ncc) = (4, 0) and (14, 4).
+BIAS_F32 with one partial per tile) and the sampling epilogue for both codebook layouts (C, ncc) = (4, 0) and (14, 4)
+at vocab_size 1024, and at vocab sizes 256 (one predicted codebook), 512 (three) and 768 (seven).
 
 The input builders and library wrappers here are shared with tests/test_gpu_gemm_fused.py.
 """
@@ -31,7 +33,7 @@ if ROOT not in sys.path:
 
 N_SAMPLE = 256
 EPS = 1e-6
-V = 1024
+V = 1024                    # the vocabulary size of the sampling cases unless a case names another
 SENTINEL_F32 = 0x7FBADBAD   # NaN bit patterns that no kernel produces: a missed or stray store shows up
 SENTINEL_BF16 = 0x7FA5
 
@@ -78,9 +80,10 @@ def untouched(t):
     return t.view(torch.int32) == SENTINEL_F32
 
 
-def sample_inputs(M, C, ncc, g):
-    """zcur (M, C) int32 on cuda:0: conditioning codebooks hold tokens; each predicted position is masked (= V) with
-    probability 0.7, and rows 32 .. 95 are known in every codebook (whole epilogue warps with nothing to sample)."""
+def sample_inputs(M, C, ncc, g, V=V):
+    """zcur (M, C) int32 on cuda:0: conditioning codebooks hold tokens; each predicted position is masked (= V, the mask
+    token) with probability 0.7, and rows 32 .. 95 are known in every codebook (whole epilogue warps with nothing to
+    sample)."""
     z = torch.randint(0, V, (M, C), generator=g, dtype=torch.int32)
     masked = torch.rand(M, C, generator=g) < 0.7
     masked[:, :ncc] = False
@@ -89,14 +92,14 @@ def sample_inputs(M, C, ncc, g):
     return z.cuda()
 
 
-def tie_columns(W, bias, g, per=4):
-    """Make exact ties: in `per` strips of every 1024-column codebook block, a scaled copy of one W row and its bias
-    entry also goes to a later column of the same 128-column strip, so those logits are equal bit for bit and are the
-    strip's maximum for many rows."""
+def tie_columns(W, bias, g, per=4, V=V):
+    """Make exact ties: in `per` strips of every V-column codebook block (all of them if it has fewer), a scaled copy of
+    one W row and its bias entry also goes to a later column of the same 128-column strip, so those logits are equal
+    bit for bit and are the strip's maximum for many rows."""
     N = W.shape[0]
-    for blk in range(N // 1024):
-        for k in torch.randperm(8, generator=g)[:per].tolist():
-            base = blk * 1024 + k * 128
+    for blk in range(N // V):
+        for k in torch.randperm(V // 128, generator=g)[:per].tolist():
+            base = blk * V + k * 128
             i, j = sorted(torch.randperm(128, generator=g)[:2].tolist())
             W[base + i] = (W[base + i].float() * 4.0).bfloat16()
             W[base + j] = W[base + i]
@@ -114,7 +117,7 @@ def gemm_fused(epi, A, W, out, out2=None, bias=None, T=1, Tpad=8, ss_in=None, in
                                        L.stream_ptr()))
 
 
-def gemm_sample(A, W, bias, ss_in, inv_d, zcur, T, C, ncc, temperature, do_sample, step, seed, partials):
+def gemm_sample(A, W, bias, ss_in, inv_d, zcur, T, C, ncc, temperature, do_sample, step, seed, partials, V=V):
     L = lib()
     M, K = A.shape
     N = W.shape[0]
@@ -143,6 +146,8 @@ CASES = [
     ("resid", 256, 300, 512), ("resid", 1280, 1725, 2560),     # extra = K
     ("embed", 256, 300, 192), ("embed", 1280, 1725, 384),      # extra = K = 3 Kp
     ("sample", 256, 450, (4, 0)), ("sample", 1280, 1725, (14, 4)),   # extra = (C, ncc)
+    ("sample", 256, 450, (1, 0, 256)), ("sample", 512, 450, (4, 1, 512)),  # extra = (C, ncc, V)
+    ("sample", 1280, 1725, (9, 2, 768)),
 ]
 
 
@@ -188,20 +193,20 @@ def run_case(kind, d, M, extra):
             gemm_fused(L.EPI_BIAS_F32, A, W, out, bias=bias, out_bf16=y, ss_out=ss_out)
         outs = [out, y, ss_out]
     else:
-        C, ncc = extra
-        T = 150 if d == 256 else 575
-        N = (C - ncc) * V
+        C, ncc, Vc = extra if len(extra) == 3 else (*extra, V)
+        T = 150 if M == 450 else 575
+        N = (C - ncc) * Vc
         A, W, g = operands(M, N, d, seed)
         bias = torch.randn(N, generator=g)
         W = W.cpu()
-        tie_columns(W, bias, g)
+        tie_columns(W, bias, g, V=Vc)
         W, bias = W.cuda(), bias.cuda()
         ss, inv_d, _ = row_stats(M, d, parts, g)
-        zcur = sample_inputs(M, C, ncc, g)
+        zcur = sample_inputs(M, C, ncc, g, V=Vc)
         outs = []
         for temperature, do_sample, step in ((0.7, 1, 11), (1.0, 0, 0)):
-            rec = sentinel((M * (C - ncc) * (V // 128), 4), torch.float32)
-            gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, (1234, 5678), rec)
+            rec = sentinel((M * (C - ncc) * (Vc // 128), 4), torch.float32)
+            gemm_sample(A, W, bias, ss, inv_d, zcur, T, C, ncc, temperature, do_sample, step, (1234, 5678), rec, V=Vc)
             outs.append(rec)
     torch.cuda.synchronize()
     return [o.cpu() for o in outs]
@@ -224,11 +229,11 @@ def sample_values(outs, name):
     return flat[sample_index(flat.size, name)]
 
 
-def record():
+def record(cases=CASES):
     rec = {}
     prev = set_pair(0)
     try:
-        for case in CASES:
+        for case in cases:
             name = case_name(*case)
             outs = run_case(*case)
             rec["sha256_" + name] = np.array(digest(outs))
@@ -242,14 +247,21 @@ def record():
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--write", metavar="NPZ", required=True, help="where to store the hashes and samples")
+    ap.add_argument("--add-to", metavar="NPZ", help="keep this record's entries as they are and record only the cases "
+                    "it lacks")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs cuda:0"
-    rec = record()
     dev = torch.cuda.get_device_properties(0)
-    rec["device"] = np.array(dev.name)
+    old = dict(np.load(args.add_to)) if args.add_to else {}
+    cases = [c for c in CASES if "sha256_" + case_name(*c) not in old]
+    rec = record(cases)
+    if old:
+        rec["device_added"] = np.array(dev.name)
+    else:
+        rec["device"] = np.array(dev.name)
     os.makedirs(os.path.dirname(os.path.abspath(args.write)), exist_ok=True)
-    np.savez_compressed(args.write, **rec)
-    print(f"wrote {len(CASES)} cases to {args.write}")
+    np.savez_compressed(args.write, **old, **rec)
+    print(f"wrote {len(cases)} new cases ({len(CASES)} in all) to {args.write}")
 
 
 if __name__ == "__main__":
