@@ -581,6 +581,54 @@ int32_t vnb_mel_loss(const float* x, const float* y, int32_t B, int32_t C, int32
                      const vnb_mel_scale* scales, int32_t n_scales, double clamp_eps, double pow, double log_weight,
                      double mag_weight, void* workspace, uint64_t workspace_bytes, float* loss, float* item_loss,
                      void* stream);
+/* ---- Frechet audio distance with VGGish embeddings (the evaluation script's frechet_audio_distance with
+ *      torchvggish, use_pca=False, use_activation=False, restated on the device; DESIGN.md §14).  Nothing here
+ *      synchronises. -----
+ * The network's weights, DEVICE, in the layouts the kernels read (vampnet_b200.fad.VGGish packs a torchvggish state
+ * dict into them).  w1 (64, 9) fp32 and b1 (64) fp32: features.0.  conv_*[l], l = 0..4, features.3, 6, 8, 11, 13:
+ * weights (Cout, 3, 3, Cin) as (Cout, 9 Cin) split bf16, x = hi + lo, and bias (Cout) fp32.  fc_*[l], l = 0..2,
+ * embeddings.0, 2, 4: weights (N, K) split bf16 with K in NHWC order, and bias (N) fp32.  The handle keeps the
+ * pointers, not copies: the buffers must outlive it. */
+typedef struct vnb_vggish_weights {
+  const float* w1;
+  const float* b1;
+  const void* conv_hi[5];
+  const void* conv_lo[5];
+  const float* conv_b[5];
+  const void* fc_hi[3];
+  const void* fc_lo[3];
+  const float* fc_b[3];
+} vnb_vggish_weights;
+/* Refused: a NULL pointer, a pointer that is not 16-byte aligned. */
+int32_t vnb_vggish_create(const vnb_vggish_weights* w, void** handle);
+void vnb_vggish_destroy(void* handle);
+/* samples (rows, N) fp32 DEVICE, mono at 16 kHz -> examples (rows * n_ex, 96, 64) fp32 DEVICE, n_ex = 1 + (F - 96) //
+ * 96 with F = 1 + (N - 400) // 160: vggish_input.waveform_to_examples after the resample, in float64 (window 400 of a
+ * 512-point FFT, hop 160, |rfft| on the 64-band HTK matrix over 125..7500 Hz, log(mel + 0.01)), rounded to fp32 once.
+ * The window, twiddles and mel matrix are built on the host in float64 on the first call on a device and cached.
+ * Refused: a NULL buffer, rows outside 1..65535, N < 15600 (no example). */
+int32_t vnb_vggish_frontend(const float* samples, int32_t rows, int32_t N, float* examples, void* stream);
+/* examples (n_ex, 96, 64) fp32 DEVICE -> embeddings (n_ex, 128) fp32 DEVICE: VGGish's features and embeddings without
+ * the final ReLU, split-bf16 tensor-core products into fp32 accumulators.  An example's embedding depends on that
+ * example only, so it equals the example run alone, bit for bit.  workspace: DEVICE, at least
+ * vnb_vggish_workspace_bytes(n_ex) bytes.  Refused: a NULL handle or buffer, n_ex outside 1..65535, a workspace that is
+ * too small. */
+int32_t vnb_vggish_workspace_bytes(int32_t n_ex, uint64_t* bytes);
+int32_t vnb_vggish_embed(void* handle, const float* examples, int32_t n_ex, void* workspace, uint64_t workspace_bytes,
+                         float* embeddings, void* stream);
+/* embeddings (M, 128) fp32 DEVICE -> mu (128) and sigma (128, 128) float64 DEVICE: np.mean(axis=0) and
+ * np.cov(rowvar=False), every sum over the rows in row order (the result does not depend on how the rows were
+ * computed or batched).  Refused: a NULL buffer, M < 2. */
+int32_t vnb_fad_moments(const float* embeddings, int64_t M, double* mu, double* sigma, void* stream);
+/* test hook: one layer of vnb_vggish_embed on DEVICE buffers.  W == 0 and Cin == 1: the first layer, x (Bn, 96, 64)
+ * fp32 and w (64, 9) fp32 -> (Bn, 48, 32, 64) hi/lo.  W > 0: a 3x3 convolution of (Bn, H, W, Cin) hi/lo with weights
+ * (N, 9 Cin) hi/lo, relu(+ bias), pooled 2x2 when pool != 0, -> hi/lo; H * W a multiple of 128 or H * W < 128 with
+ * 128 / W even.  W == 0 and Cin > 1: a fully connected layer of (Bn, Cin) hi/lo with weights (N, Cin) hi/lo: relu != 0
+ * -> relu(+ bias) hi/lo, relu == 0 -> (+ bias) fp32 out_f32.  N a multiple of 128, Cin a multiple of 64.  Refused: a
+ * NULL buffer, a shape outside these. */
+int32_t vnb_dbg_vggish_layer(const float* x, const float* w, const void* a_hi, const void* a_lo, int32_t Bn, int32_t H,
+                             int32_t W, int32_t Cin, const void* w_hi, const void* w_lo, int32_t N, const float* bias,
+                             int32_t relu, int32_t pool, void* out_hi, void* out_lo, float* out_f32, void* stream);
 /* internal helper exported for the other translation units */
 int32_t vnb_set_error_cuda(const char* what, int32_t cuda_error);
 

@@ -64,6 +64,12 @@ class MelScale(C.Structure):
                 ("fmax", C.c_double)]
 
 
+class VggishWeights(C.Structure):
+    _fields_ = [("w1", C.c_void_p), ("b1", C.c_void_p), ("conv_hi", C.c_void_p * 5), ("conv_lo", C.c_void_p * 5),
+                ("conv_b", C.c_void_p * 5), ("fc_hi", C.c_void_p * 3), ("fc_lo", C.c_void_p * 3),
+                ("fc_b", C.c_void_p * 3)]
+
+
 _SIGS = {
     "vnb_abi_version": (C.c_int32, []),
     "vnb_last_error": (C.c_char_p, []),
@@ -169,6 +175,16 @@ _SIGS = {
     "vnb_mel_workspace_bytes": (C.c_int32, [C.c_int32] * 4 + [C.POINTER(MelScale), C.c_int32, C.POINTER(C.c_uint64)]),
     "vnb_mel_loss": (C.c_int32, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.POINTER(MelScale), C.c_int32] + [C.c_double] * 4
                      + [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_vggish_create": (C.c_int32, [C.POINTER(VggishWeights), C.POINTER(C.c_void_p)]),
+    "vnb_vggish_destroy": (None, [C.c_void_p]),
+    "vnb_vggish_frontend": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vnb_vggish_workspace_bytes": (C.c_int32, [C.c_int32, C.POINTER(C.c_uint64)]),
+    "vnb_vggish_embed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p,
+                                     C.c_void_p]),
+    "vnb_fad_moments": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vnb_dbg_vggish_layer": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_int32, C.c_void_p,
+                                                                                        C.c_int32, C.c_int32]
+                             + [C.c_void_p] * 4),
     "vnb_dbg_sample": (C.c_int32, [C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup),
                                                                                         C.c_int32, C.c_void_p]),
     "vnb_dbg_sample_split": (C.c_int32, [C.c_void_p] * 7 + [C.c_int32] * 6 + [C.POINTER(SampleGroup), C.c_int32,

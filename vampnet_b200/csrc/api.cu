@@ -93,6 +93,28 @@ bool make_tmap_3d(CUtensorMap* tm, const void* base, uint64_t batch, uint64_t ro
   return true;
 }
 
+bool make_tmap_4d(CUtensorMap* tm, const void* base, uint64_t batch, uint64_t H, uint64_t W, uint64_t C,
+                  uint32_t box_h, uint32_t box_c) {
+  auto enc = get_encode();
+  if (!enc) return false;
+  cuuint64_t dims[4] = {C, W, H, batch};
+  cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
+  cuuint32_t box[4] = {box_c, static_cast<cuuint32_t>(W), box_h, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char b[256];
+    snprintf(b, sizeof(b), "cuTensorMapEncodeTiled(4d batch=%llu H=%llu W=%llu C=%llu box=%ux%llux%u) -> %d",
+             (unsigned long long)batch, (unsigned long long)H, (unsigned long long)W, (unsigned long long)C, box_h,
+             (unsigned long long)W, box_c, (int)r);
+    g_tmap_err = b;
+    return false;
+  }
+  return true;
+}
+
 // Fills a plan's tensor maps (A (M,K) bf16, W (N,K) bf16) and arguments, with the fused RMSNorm (DESIGN.md §4) wired as
 // in the forward: ss_in (non-null) makes the plan a consumer that scales its rows by rsqrt(mean(A^2) + eps) from ss_parts
 // partial row sums of squares; out_bf16 (non-null) a producer that also stores bf16(out) and its row sums of squares
@@ -647,7 +669,6 @@ static int fused_sampler_enabled() {
   }
   return g_fused_sampler;
 }
-
 }  // extern "C"
 
 // v.mixed_steps: iteration i runs only the batch rows ws->live[i] counts (a prefix); the others are idle and untouched.
@@ -1454,6 +1475,88 @@ int32_t vnb_mel_loss(const float* x, const float* y, int32_t B, int32_t C, int32
   if (int32_t rc = check_workspace("vnb_mel_loss", workspace_bytes, p.total)) return rc;
   CK(launch_mel_loss(x, y, p, clamp_eps, pow, log_weight, mag_weight, workspace, loss, item_loss,
                      reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+// ---- Frechet audio distance with VGGish embeddings (fad.cu) ----
+int32_t vnb_vggish_create(const vnb_vggish_weights* w, void** handle) {
+  if (!w || !handle) return fail("vnb_vggish_create: weights and handle are required");
+  std::vector<std::pair<const char*, const void*>> ptrs = {{"w1", w->w1}, {"b1", w->b1}};
+  static const char* conv_names[5] = {"conv 0", "conv 1", "conv 2", "conv 3", "conv 4"};
+  static const char* fc_names[3] = {"fc 0", "fc 1", "fc 2"};
+  for (int l = 0; l < 5; ++l) {
+    ptrs.push_back({conv_names[l], w->conv_hi[l]}); ptrs.push_back({conv_names[l], w->conv_lo[l]});
+    ptrs.push_back({conv_names[l], w->conv_b[l]});
+  }
+  for (int l = 0; l < 3; ++l) {
+    ptrs.push_back({fc_names[l], w->fc_hi[l]}); ptrs.push_back({fc_names[l], w->fc_lo[l]});
+    ptrs.push_back({fc_names[l], w->fc_b[l]});
+  }
+  for (const auto& p : ptrs) {
+    if (!p.second) return fail("vnb_vggish_create: %s: a weight pointer is NULL", p.first);
+    if (reinterpret_cast<uintptr_t>(p.second) % 16) return fail("vnb_vggish_create: %s: a weight pointer is not 16-byte aligned", p.first);
+  }
+  VggishNet* net = new VggishNet;
+  net->w1 = w->w1; net->b1 = w->b1;
+  for (int l = 0; l < 5; ++l) { net->conv_hi[l] = w->conv_hi[l]; net->conv_lo[l] = w->conv_lo[l]; net->conv_b[l] = w->conv_b[l]; }
+  for (int l = 0; l < 3; ++l) { net->fc_hi[l] = w->fc_hi[l]; net->fc_lo[l] = w->fc_lo[l]; net->fc_b[l] = w->fc_b[l]; }
+  *handle = net;
+  return 0;
+}
+void vnb_vggish_destroy(void* handle) { delete static_cast<VggishNet*>(handle); }
+int32_t vnb_vggish_frontend(const float* samples, int32_t rows, int32_t N, float* examples, void* stream) {
+  if (!samples || !examples) return fail("vnb_vggish_frontend: samples and examples are required");
+  if (rows < 1 || rows > 65535) return fail("vnb_vggish_frontend: need 1 <= rows <= 65535 (got %d)", rows);
+  if (vggish_examples(N) < 1) return fail("vnb_vggish_frontend: N = %d samples at 16 kHz give no example (15600 needed)", N);
+  CK(launch_vggish_frontend(samples, rows, N, examples, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_vggish_workspace_bytes(int32_t n_ex, uint64_t* bytes) {
+  if (!bytes) return fail("vnb_vggish_workspace_bytes: bytes is NULL");
+  if (n_ex < 1 || n_ex > 65535) return fail("vnb_vggish_workspace_bytes: need 1 <= n_ex <= 65535 (got %d)", n_ex);
+  *bytes = vggish_workspace_bytes(n_ex);
+  return 0;
+}
+int32_t vnb_vggish_embed(void* handle, const float* examples, int32_t n_ex, void* workspace, uint64_t workspace_bytes,
+                         float* embeddings, void* stream) {
+  if (!handle || !examples || !workspace || !embeddings)
+    return fail("vnb_vggish_embed: handle, examples, workspace and embeddings are required");
+  if (n_ex < 1 || n_ex > 65535) return fail("vnb_vggish_embed: need 1 <= n_ex <= 65535 (got %d)", n_ex);
+  if (int32_t rc = check_workspace("vnb_vggish_embed", workspace_bytes, vggish_workspace_bytes(n_ex))) return rc;
+  const cudaError_t e = launch_vggish_embed(*static_cast<const VggishNet*>(handle), examples, n_ex, workspace,
+                                            embeddings, reinterpret_cast<cudaStream_t>(stream));
+  if (e == cudaErrorInvalidValue && tmap_error()[0]) return fail("vnb_vggish_embed: %s", tmap_error());
+  CK(e);
+  return 0;
+}
+int32_t vnb_fad_moments(const float* embeddings, int64_t M, double* mu, double* sigma, void* stream) {
+  if (!embeddings || !mu || !sigma) return fail("vnb_fad_moments: embeddings, mu and sigma are required");
+  if (M < 2) return fail("vnb_fad_moments: need M >= 2 embeddings (got %lld)", (long long)M);
+  CK(launch_fad_moments(embeddings, M, mu, sigma, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int32_t vnb_dbg_vggish_layer(const float* x, const float* w, const void* a_hi, const void* a_lo, int32_t Bn, int32_t H,
+                             int32_t W, int32_t Cin, const void* w_hi, const void* w_lo, int32_t N, const float* bias,
+                             int32_t relu, int32_t pool, void* out_hi, void* out_lo, float* out_f32, void* stream) {
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (Bn < 1 || Bn > 65535 || !bias) return fail("vnb_dbg_vggish_layer: need 1 <= Bn <= 65535 and a bias");
+  if (W == 0 && Cin == 1) {
+    if (!x || !w || !out_hi || !out_lo) return fail("vnb_dbg_vggish_layer: x, w, out_hi and out_lo are required");
+    CK(launch_vggish_in(x, w, bias, Bn, out_hi, out_lo, st));
+    return 0;
+  }
+  if (!a_hi || !a_lo || !w_hi || !w_lo) return fail("vnb_dbg_vggish_layer: a_hi, a_lo, w_hi and w_lo are required");
+  if (N < 128 || N % 128 || Cin < 64 || Cin % 64) return fail("vnb_dbg_vggish_layer: need N % 128 == 0 and Cin % 64 == 0");
+  if (W > 0) {
+    if (W > 128 || 128 % W || (128 / W) % 2 || H < 2 || H % 2 || (H * W > 128 && (H * W) % 128) || !out_hi || !out_lo)
+      return fail("vnb_dbg_vggish_layer: unsupported image %d x %d", H, W);
+  } else if (relu ? (!out_hi || !out_lo) : !out_f32) {
+    return fail("vnb_dbg_vggish_layer: the output is required");
+  }
+  const cudaError_t e = launch_vggish_tc(a_hi, a_lo, Bn, H, W, Cin, w_hi, w_lo, N, bias, W > 0 || relu, W > 0 && pool,
+                                         out_hi, out_lo, out_f32, st);
+  if (e == cudaErrorInvalidValue) return fail("vnb_dbg_vggish_layer: %s", tmap_error());
+  CK(e);
   return 0;
 }
 

@@ -18,6 +18,12 @@
 // Epilogue (fused): + bias, + fp32 skip (residual units), store the fp32 stream, and/or apply the NEXT layer's
 // Snake activation (x + sin^2(alpha x)/alpha) and store it split as hi/lo bf16 = the next conv's A operand.
 //
+// VGGish (fad.cu) runs its 3x3 convolutions and fully connected layers through the same kernel.  A 2-D convolution
+// (g.W > 0) reads NHWC images (Bn, H, W, Cin): a 128-row tile is 128 / W whole image rows, and the A box of tap (dh, dw)
+// is a 4-D TMA box at (h0 + dh - 1, w0 + dw - 1) whose out-of-bounds zero fill is the padding on both axes.  Its
+// epilogue adds the bias and applies ReLU, and with the 2 x 2 max-pool (an even number of image rows per tile) stores
+// the pooled (H/2, W/2) image, split hi/lo.
+//
 // Same warp-specialised structure as gemm_wgmma.cu: TMA producer warp, two consumer warpgroups (64 rows x NW columns
 // of wgmma accumulators each), one CTA per tile of 128 rows x BN columns (BN <= 128, runtime).  The MMA width NW is
 // the narrowest of 32 / 64 / 128 that covers BN, so the narrow audio-rate layers issue no MMAs for columns they do not
@@ -55,6 +61,8 @@ struct ConvTcArgs {
   // Clips of different lengths in one launch (vnb_codec_conv_tc_ragged): DEVICE [Bn] valid output rows of each item,
   // in rows of row_elems elements (N for a plain convolution, Cout for a transposed one).  NULL: every item is Tq rows.
   const int* lens; int row_elems;
+  // CT_RELU / CT_RELU_POOL: image height and width of a 2-D convolution (Tq = H * W), W = 0 for 1-D addressing
+  int H, W;
 };
 
 // Halo of a ragged launch: rows [len_b, len_b + CT_HALO) of every output hold +0, so that the next layer's valid rows
@@ -82,7 +90,9 @@ __device__ __forceinline__ float snake_act(float v, float a, float inv_a) {
 //   CT_SPLIT        y -> snake_next(y) -> hi/lo                                  (k = 7 convolution of a residual unit)
 //   CT_SPLIT_SKIP   y + skip -> fp32 stream (in place) and snake_next -> hi/lo   (1 x 1 convolution closing the unit)
 //   CT_SPLIT_F32    y -> fp32 stream and snake_next -> hi/lo                     (strided / transposed convolutions)
-enum : int { CT_GENERIC = 0, CT_SPLIT = 1, CT_SPLIT_SKIP = 2, CT_SPLIT_F32 = 3 };
+//   CT_RELU         relu(y + bias) -> hi/lo                         (VGGish: 3x3 convolutions without a pool, FC 1-2)
+//   CT_RELU_POOL    2x2 max-pool of relu(y + bias) -> hi/lo         (VGGish: 3x3 convolutions followed by a pool)
+enum : int { CT_GENERIC = 0, CT_SPLIT = 1, CT_SPLIT_SKIP = 2, CT_SPLIT_F32 = 3, CT_RELU = 4, CT_RELU_POOL = 5 };
 
 template <int MODE, int NW>
 __global__ void __launch_bounds__(CT_THREADS, 1)
@@ -134,8 +144,14 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sa = smem + stage * CT_STAGE_BYTES;
         mbar_expect_tx(&full_bar[stage], stage_tx);
-        tma_load_3d(sa, &tmAh, &full_bar[stage], col, q0 + qs, b);
-        tma_load_3d(sa + CT_A_BYTES, &tmAl, &full_bar[stage], col, q0 + qs, b);
+        if (MODE >= CT_RELU && g.W > 0) {  // 2-D 3x3 convolution: tap = 3 dh + dw
+          const int h = q0 / g.W + tap / 3 - 1, w = tap % 3 - 1;
+          tma_load_4d(sa, &tmAh, &full_bar[stage], cblk * CT_BK, w, h, b);
+          tma_load_4d(sa + CT_A_BYTES, &tmAl, &full_bar[stage], cblk * CT_BK, w, h, b);
+        } else {
+          tma_load_3d(sa, &tmAh, &full_bar[stage], col, q0 + qs, b);
+          tma_load_3d(sa + CT_A_BYTES, &tmAl, &full_bar[stage], col, q0 + qs, b);
+        }
         tma_load_2d(sa + 2 * CT_A_BYTES, &tmWh, &full_bar[stage], kb * CT_BK, n0);
         tma_load_2d(sa + 2 * CT_A_BYTES + CT_B_BYTES, &tmWl, &full_bar[stage], kb * CT_BK, n0);
         if (++stage == CT_STAGES) { stage = 0; phase ^= 1; }
@@ -229,9 +245,42 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
 
   // ===================== epilogue =====================
   const uint32_t acc_tile = smem_u32(smem);
-  const bool out_f32 = MODE == CT_GENERIC ? g.out_f32 != nullptr : MODE != CT_SPLIT;
-  const bool out_split = MODE == CT_GENERIC ? g.out_hi != nullptr : true;
-  const bool snake = MODE == CT_GENERIC ? g.alpha != nullptr : true;
+  if constexpr (MODE == CT_RELU_POOL) {
+    // pooled pixel p of this tile's (128 / W / 2) x (W / 2), four columns per thread; relu(max(.) + bias) equals the
+    // max of relu(. + bias)
+    const int W2 = g.W / 2, H2 = g.H / 2, nq = g.BN / 4;
+    const int ph0 = q0 / g.W / 2;
+    for (int i = threadIdx.x; i < (CT_BM / 4) * nq; i += 32 * CT_EPI_WARPS) {
+      const int p = i / nq, cq = (i - p * nq) * 4, n = n0 + cq;
+      const int ph = p / W2, pw = p - ph * W2;
+      if (ph0 + ph >= H2 || n >= g.N) continue;
+      const int r = 2 * ph * g.W + 2 * pw;
+      const float4 bv = __ldg(reinterpret_cast<const float4*>(g.bias + n));
+      float v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t sp = acc_tile + 4u * (r * CT_ACC_PITCH + cq + j);
+        const float m = fmaxf(fmaxf(lds_f32(sp), lds_f32(sp + 4u * CT_ACC_PITCH)),
+                              fmaxf(lds_f32(sp + 4u * (g.W * CT_ACC_PITCH)), lds_f32(sp + 4u * ((g.W + 1) * CT_ACC_PITCH))));
+        v[j] = fmaxf(m + (&bv.x)[j], 0.f);
+      }
+      const __nv_bfloat162 h01 = __floats2bfloat162_rn(v[0], v[1]), h23 = __floats2bfloat162_rn(v[2], v[3]);
+      const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
+      uint2 hi, lo;
+      hi.x = *reinterpret_cast<const uint32_t*>(&h01);
+      hi.y = *reinterpret_cast<const uint32_t*>(&h23);
+      lo.x = pack_bf16x2(v[0] - f01.x, v[1] - f01.y);
+      lo.y = pack_bf16x2(v[2] - f23.x, v[3] - f23.y);
+      const long long o = static_cast<long long>(b) * g.out_batch_stride +
+                          (static_cast<long long>(ph0 + ph) * W2 + pw) * g.N + n;
+      *reinterpret_cast<uint2*>(g.out_hi + o) = hi;
+      *reinterpret_cast<uint2*>(g.out_lo + o) = lo;
+    }
+    return;
+  }
+  const bool out_f32 = MODE == CT_GENERIC || MODE == CT_RELU ? g.out_f32 != nullptr : MODE != CT_SPLIT;
+  const bool out_split = MODE == CT_GENERIC || MODE == CT_RELU ? g.out_hi != nullptr : true;
+  const bool snake = MODE == CT_GENERIC ? g.alpha != nullptr : MODE != CT_RELU;
   const bool do_tanh = MODE == CT_GENERIC ? g.do_tanh != 0 : false;
   const bool has_bias = MODE == CT_GENERIC ? g.bias != nullptr : true;
   const long long bbase = static_cast<long long>(b) * g.out_batch_stride;
@@ -268,6 +317,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constan
             a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
           }
           if (do_tanh) { a.x = tanhf(a.x); a.y = tanhf(a.y); a.z = tanhf(a.z); a.w = tanhf(a.w); }
+          if (MODE == CT_RELU) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
           if (halo) a = make_float4(0.f, 0.f, 0.f, 0.f);
           if (out_f32) *reinterpret_cast<float4*>(g.out_f32 + o) = a;
           if (out_split) {
@@ -444,6 +494,108 @@ static cudaError_t launch_conv(const CUtensorMap& tAh, const CUtensorMap& tAl, c
   else if (fast && !resid && out_f32) conv_wgmma_kernel<CT_SPLIT_F32, NW><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
   else if (fast && !resid && !out_f32) conv_wgmma_kernel<CT_SPLIT, NW><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
   else conv_wgmma_kernel<CT_GENERIC, NW><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// VGGish's first layer on CUDA cores (Cin = 1, K = 9: 0.4 % of the network's FLOPs): examples (Bn, 96, 64) fp32 ->
+// relu(3x3 conv, pad 1, + bias) -> 2x2 max-pool -> (Bn, 48, 32, 64) NHWC, split hi/lo.  One thread = four channels of
+// one pooled pixel: its 4x4 input patch, the four conv outputs under the pool, in fp32 with the taps in (dh, dw) order.
+__global__ void __launch_bounds__(256) vggish_in_kernel(const float* __restrict__ x, const float* __restrict__ w,
+                                                        const float* __restrict__ bias, __nv_bfloat16* __restrict__ out_hi,
+                                                        __nv_bfloat16* __restrict__ out_lo, int Bn) {
+  constexpr int H = 96, W = 64, C = 64, H2 = H / 2, W2 = W / 2, C4 = C / 4;
+  const long long pix = static_cast<long long>(blockIdx.x) * (256 / C4) + threadIdx.x / C4;  // (b, ph, pw)
+  if (pix >= static_cast<long long>(Bn) * H2 * W2) return;
+  const int c = (threadIdx.x % C4) * 4;
+  const int b = static_cast<int>(pix / (H2 * W2)), rem = static_cast<int>(pix % (H2 * W2));
+  const int h0 = (rem / W2) * 2 - 1, w0 = (rem % W2) * 2 - 1;
+  const float* xb = x + static_cast<long long>(b) * H * W;
+  float patch[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int h = h0 + i, ww = w0 + j;
+      patch[i][j] = (h >= 0 && h < H && ww >= 0 && ww < W) ? __ldg(xb + h * W + ww) : 0.f;
+    }
+  float v[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float bk = __ldg(bias + c + k);
+    float m = -INFINITY;
+#pragma unroll
+    for (int oy = 0; oy < 2; ++oy)
+#pragma unroll
+      for (int ox = 0; ox < 2; ++ox) {
+        float acc = bk;
+#pragma unroll
+        for (int t = 0; t < 9; ++t) acc = fmaf(__ldg(w + (c + k) * 9 + t), patch[oy + t / 3][ox + t % 3], acc);
+        m = fmaxf(m, acc);
+      }
+    v[k] = fmaxf(m, 0.f);
+  }
+  const __nv_bfloat162 h01 = __floats2bfloat162_rn(v[0], v[1]), h23 = __floats2bfloat162_rn(v[2], v[3]);
+  const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
+  uint2 hi, lo;
+  hi.x = *reinterpret_cast<const uint32_t*>(&h01);
+  hi.y = *reinterpret_cast<const uint32_t*>(&h23);
+  lo.x = pack_bf16x2(v[0] - f01.x, v[1] - f01.y);
+  lo.y = pack_bf16x2(v[2] - f23.x, v[3] - f23.y);
+  const long long o = pix * C + c;
+  *reinterpret_cast<uint2*>(out_hi + o) = hi;
+  *reinterpret_cast<uint2*>(out_lo + o) = lo;
+}
+
+cudaError_t launch_vggish_in(const float* x, const float* w, const float* bias, int Bn, void* out_hi, void* out_lo,
+                             cudaStream_t st) {
+  const long long pix = static_cast<long long>(Bn) * 48 * 32;
+  vggish_in_kernel<<<static_cast<unsigned>((pix + 15) / 16), 256, 0, st>>>(
+      x, w, bias, reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), Bn);
+  count_launch();
+  return cudaGetLastError();
+}
+
+// One VGGish layer on the tensor cores at 128-column tiles (every N is a multiple of 128): a 3x3 convolution (W > 0:
+// A = (Bn, H, W, Cin) NHWC, pool selects CT_RELU_POOL) or a fully connected layer (W = 0: A = (M, K) = (Bn, Cin), relu
+// selects CT_RELU with hi/lo output, else fp32 output without activation).  TMA maps that cannot be encoded return
+// cudaErrorInvalidValue with tmap_error() set.
+cudaError_t launch_vggish_tc(const void* a_hi, const void* a_lo, int Bn, int H, int W, int Cin, const void* w_hi,
+                             const void* w_lo, int N, const float* bias, bool relu, bool pool, void* out_hi,
+                             void* out_lo, float* out_f32, cudaStream_t st) {
+  static PerDeviceOnce once;
+  int dev;
+  if (once.need(&dev)) {
+    cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<CT_RELU, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgmma_kernel<CT_RELU_POOL, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgmma_kernel<CT_GENERIC, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM);
+    if (e != cudaSuccess) return e;
+    once.mark(dev);
+  }
+  ConvTcArgs g{};
+  const bool conv = W > 0;
+  g.Bn = conv ? Bn : 1; g.Tq = conv ? H * W : Bn; g.N = N; g.BN = 128;
+  g.cblocks = (Cin + CT_BK - 1) / CT_BK; g.taps = conv ? 9 : 1; g.dil = 1; g.pad = 0; g.s = 1; g.Cin = Cin;
+  g.bias = bias; g.bias_mod = N;
+  g.out_hi = relu ? reinterpret_cast<__nv_bfloat16*>(out_hi) : nullptr;
+  g.out_lo = relu ? reinterpret_cast<__nv_bfloat16*>(out_lo) : nullptr;
+  g.out_f32 = relu ? nullptr : out_f32;
+  g.out_batch_stride = static_cast<long long>(pool ? (H / 2) * (W / 2) : g.Tq) * N;
+  g.out_limit = static_cast<long long>(g.Tq) * N;
+  g.H = conv ? H : 0; g.W = conv ? W : 0;
+  CUtensorMap tAh, tAl, tWh, tWl;
+  const int Ktot = g.taps * g.cblocks * CT_BK;
+  const bool ok = conv ? make_tmap_4d(&tAh, a_hi, Bn, H, W, Cin, CT_BM / W, CT_BK) &&
+                             make_tmap_4d(&tAl, a_lo, Bn, H, W, Cin, CT_BM / W, CT_BK)
+                       : make_tmap_3d(&tAh, a_hi, 1, Bn, Cin, Cin, CT_BM, CT_BK) &&
+                             make_tmap_3d(&tAl, a_lo, 1, Bn, Cin, Cin, CT_BM, CT_BK);
+  if (!ok || !make_tmap_2d(&tWh, w_hi, N, Ktot, g.BN, CT_BK) || !make_tmap_2d(&tWl, w_lo, N, Ktot, g.BN, CT_BK))
+    return cudaErrorInvalidValue;
+  const dim3 grid(g.Bn * ((g.Tq + CT_BM - 1) / CT_BM) * (N / g.BN));
+  if (pool) conv_wgmma_kernel<CT_RELU_POOL, 128><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
+  else if (relu) conv_wgmma_kernel<CT_RELU, 128><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
+  else conv_wgmma_kernel<CT_GENERIC, 128><<<grid, CT_THREADS, CT_SMEM, st>>>(tAh, tAl, tWh, tWl, g);
+  count_launch();
   return cudaGetLastError();
 }
 

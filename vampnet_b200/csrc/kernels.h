@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <functional>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/vampnet_b200.h"
@@ -47,7 +48,7 @@ inline size_t carve(size_t& o, size_t bytes) {
 // Constant device tables (tables.cu): the table named by `key` (its kind, then the parameters its values depend on) is
 // built on the host by `build` once per (current device, key), uploaded, and kept for the life of the process; *dev
 // receives its device copy.
-enum TableKind { TABLE_FFT, TABLE_MEL_BANK, TABLE_BEAT, TABLE_PITCH_BASIS };
+enum TableKind { TABLE_FFT, TABLE_MEL_BANK, TABLE_BEAT, TABLE_PITCH_BASIS, TABLE_VGGISH_FFT, TABLE_VGGISH_HTK };
 cudaError_t device_table(const std::vector<double>& key, const std::function<std::vector<char>()>& build,
                          const char** dev);
 
@@ -58,6 +59,9 @@ bool make_tmap_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t col
 // 3-D bf16 (batch, rows, cols) row-major with row pitch `pitch_elems`; box (1, box_rows, 64), 128B swizzle.
 bool make_tmap_3d(CUtensorMap* tm, const void* base, uint64_t batch, uint64_t rows, uint64_t cols,
                   uint64_t pitch_elems, uint32_t box_rows, uint32_t box_cols);
+// 4-D bf16 NHWC images (batch, H, W, C); box (1, box_h, W, box_c) of whole image rows, 128B swizzle.
+bool make_tmap_4d(CUtensorMap* tm, const void* base, uint64_t batch, uint64_t H, uint64_t W, uint64_t C,
+                  uint32_t box_h, uint32_t box_c);
 const char* tmap_error();
 }  // namespace vnb
 // sets the thread-local error string from a CUDA error code; returns 1
@@ -203,27 +207,46 @@ cudaError_t launch_remask_dev(const SampleArgs& a, const SampleDyn* dyn_dev, cud
 // groups from `partials`, the nucleus draw the rows of top-p groups from a.logits, then the re-mask
 cudaError_t launch_sample_split_dev(const SampleArgs& a, const void* partials, const SampleDyn* dyn_dev, cudaStream_t st);
 
-// ---- spectrogram tables (mel.cu): built in float64, rounded to fp32 once, cached by device_table ----
-struct FftTables {
-  const float2* twiddle;  // (n_fft / 2 + 1) exp(-2 pi i k / n_fft), for fft.cuh
-  const float* window;    // (n_fft) periodic Hann
+// ---- spectrogram tables (mel.cu): built in float64, rounded to the kernel's scalar type R once, cached by device_table ----
+template <typename R>
+using Complex = typename std::conditional<std::is_same<R, double>::value, double2, float2>::type;
+template <typename R>
+struct FftTablesT {
+  const Complex<R>* twiddle;  // (n_fft / 2 + 1) exp(-2 pi i k / n_fft), for fft.cuh
+  const R* window;            // (n_fft) periodic Hann (VGGish: of length 400, zero-extended)
 };
+using FftTables = FftTablesT<float>;
 cudaError_t fft_tables(int n_fft, FftTables* out);  // per (device, n_fft)
-// librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm="slaney", dtype=float32), nonzero ranges only
-struct MelBank {
-  const float* w;       // band m's weights at [off[m], off[m + 1]), for bins lo[m], lo[m] + 1, ...
+// a filterbank's nonzero ranges: librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm="slaney",
+// dtype=float32) for the fp32 modes, VGGish's HTK matrix for VGGISH_LOG
+template <typename R>
+struct MelBankT {
+  const R* w;           // band m's weights at [off[m], off[m + 1]), for bins lo[m], lo[m] + 1, ...
   const int32_t* off;   // (n_mels + 1)
   const int32_t* lo;    // (n_mels) first nonzero bin of band m (0 for an empty band)
 };
+using MelBank = MelBankT<float>;
 cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fmax, MelBank* out);  // per (device, all)
 
-// The spectrogram kernel's two outputs from samples (rows, N) fp32, F = 1 + N / hop frames:
-//   ONSET_DB  onset detection's: zero padding (any N >= 1), ONSET_NFFT points, |X|^2 on ONSET_NMELS bands, then
-//             10 log10(max(1e-10, s)); (rows, F, ONSET_NMELS)
-//   MEL_MAG   the mel distance's: reflect padding (N > n_fft / 2), n_fft a power of two in MEL_MIN_NFFT..MEL_MAX_NFFT,
-//             |X| on n_mels bands; (rows, n_mels, F)
-enum class SpecMode { ONSET_DB, MEL_MAG };
+// The spectrogram kernel's outputs from samples (rows, N) fp32:
+//   ONSET_DB    onset detection's: F = 1 + N / hop frames, zero padding (any N >= 1), ONSET_NFFT points, |X|^2 on
+//               ONSET_NMELS bands, then 10 log10(max(1e-10, s)); (rows, F, ONSET_NMELS)
+//   MEL_MAG     the mel distance's: F = 1 + N / hop frames, reflect padding (N > n_fft / 2), n_fft a power of two in
+//               MEL_MIN_NFFT..MEL_MAX_NFFT, |X| on n_mels bands; (rows, n_mels, F)
+//   VGGISH_LOG  VGGish's log-mel examples (fad.cu), in float64: no padding, a VGGISH_WIN-point window in a VGGISH_NFFT-point
+//               FFT, hop VGGISH_HOP, |X| on the VGGISH_NMELS-band HTK matrix, log(s + 0.01) rounded to fp32 once; the
+//               first n_ex(N) * VGGISH_EX_FRAMES frames of each row, (rows * n_ex, VGGISH_EX_FRAMES, VGGISH_NMELS)
+enum class SpecMode { ONSET_DB, MEL_MAG, VGGISH_LOG };
 constexpr int ONSET_NFFT = 2048, ONSET_NMELS = 128;
+constexpr int VGGISH_SR = 16000, VGGISH_WIN = 400, VGGISH_HOP = 160, VGGISH_NFFT = 512, VGGISH_NMELS = 64;
+constexpr int VGGISH_EX_FRAMES = 96;
+constexpr double VGGISH_FMIN = 125.0, VGGISH_FMAX = 7500.0;
+// examples of N samples at 16 kHz: 1 + (F - 96) // 96 with F = 1 + (N - 400) // 160 frames; 0 below 15600 samples
+inline int vggish_examples(long long N) {
+  if (N < VGGISH_WIN) return 0;
+  const long long F = 1 + (N - VGGISH_WIN) / VGGISH_HOP;
+  return F < VGGISH_EX_FRAMES ? 0 : (int)(1 + (F - VGGISH_EX_FRAMES) / VGGISH_EX_FRAMES);
+}
 cudaError_t launch_spectrogram(SpecMode mode, const float* samples, int rows, int N, int hop, int n_fft,
                                const FftTables& fft, const MelBank& bank, int n_mels, float* out, cudaStream_t st);
 
@@ -334,5 +357,28 @@ cudaError_t launch_mel_spectrogram(const float* samples, int rows, int N, int sr
 cudaError_t launch_mel_loss(const float* x, const float* y, const MelLossPlan& p, double clamp_eps, double pow,
                             double log_weight, double mag_weight, void* workspace, float* loss, float* item_loss,
                             cudaStream_t st);
+
+// ---- Frechet audio distance with VGGish embeddings (fad.cu, conv_wgmma.cu, mel.cu; DESIGN.md §14) ----
+// samples (rows, N) fp32 at 16 kHz -> (rows * vggish_examples(N), 96, 64) fp32 log-mel examples (SpecMode::VGGISH_LOG)
+cudaError_t launch_vggish_frontend(const float* samples, int rows, int N, float* out, cudaStream_t st);
+// layer 1: examples (Bn, 96, 64) fp32, w (64, 9) fp32 -> relu, 2x2 max-pool -> (Bn, 48, 32, 64) hi/lo bf16
+cudaError_t launch_vggish_in(const float* x, const float* w, const float* bias, int Bn, void* out_hi, void* out_lo,
+                             cudaStream_t st);
+// layers 2-9 on the tensor cores (conv_wgmma_kernel's CT_RELU / CT_RELU_POOL / CT_GENERIC modes)
+cudaError_t launch_vggish_tc(const void* a_hi, const void* a_lo, int Bn, int H, int W, int Cin, const void* w_hi,
+                             const void* w_lo, int N, const float* bias, bool relu, bool pool, void* out_hi,
+                             void* out_lo, float* out_f32, cudaStream_t st);
+// the embedding network's weights, as vnb_vggish_weights holds them
+struct VggishNet {
+  const float* w1; const float* b1;
+  const void* conv_hi[5]; const void* conv_lo[5]; const float* conv_b[5];
+  const void* fc_hi[3]; const void* fc_lo[3]; const float* fc_b[3];
+};
+size_t vggish_workspace_bytes(int n_ex);
+// examples (n_ex, 96, 64) fp32 -> embeddings (n_ex, 128) fp32
+cudaError_t launch_vggish_embed(const VggishNet& net, const float* examples, int n_ex, void* workspace, float* out,
+                                cudaStream_t st);
+// embeddings (M, 128) fp32 -> mu (128) and sigma (128, 128) float64, np.mean and np.cov(rowvar=False)
+cudaError_t launch_fad_moments(const float* emb, long long M, double* mu, double* sigma, cudaStream_t st);
 
 }  // namespace vnb

@@ -34,31 +34,39 @@ struct MelGeom {
 
 constexpr int ilog2(int n) { return n <= 1 ? 0 : 1 + ilog2(n / 2); }
 
+template <typename R>
 struct MelSpecArgs {
-  FftTables fft;
-  MelBank bank;
+  FftTablesT<R> fft;
+  MelBankT<R> bank;
   int n_mels;
 };
 
 template <int NFFT, SpecMode MODE>
-__global__ void __launch_bounds__(THREADS) mel_spec_kernel(const float* __restrict__ samples, int N, int F, int hop,
-                                                           MelSpecArgs t, float* __restrict__ out) {
-  constexpr bool DB = MODE == SpecMode::ONSET_DB;
+__global__ void __launch_bounds__(THREADS)
+mel_spec_kernel(const float* __restrict__ samples, int N, int F, int hop,
+                MelSpecArgs<typename std::conditional<MODE == SpecMode::VGGISH_LOG, double, float>::type> t,
+                float* __restrict__ out) {
+  constexpr bool DB = MODE == SpecMode::ONSET_DB, VGG = MODE == SpecMode::VGGISH_LOG;
+  using R = typename std::conditional<VGG, double, float>::type;
+  using C2 = Complex<R>;
   constexpr int NH = NFFT / 2, NBINS = NH + 1, TPF = MelGeom<NFFT>::TPF, FPC = MelGeom<NFFT>::FPC;
-  __shared__ float2 zs[FPC * NH];
-  __shared__ float Ps[FPC * NBINS];
+  __shared__ C2 zs[FPC * NH];
+  __shared__ R Ps[FPC * NBINS];
   const int g = threadIdx.x / TPF, lt = threadIdx.x % TPF;
   const int f = blockIdx.x * FPC + g, row = blockIdx.y;
   const bool live = FPC == 1 || f < F;  // the last CTA's spare groups still take part in the block-wide barriers
-  float2* z = zs + g * NH;
-  float* P = Ps + g * NBINS;
+  C2* z = zs + g * NH;
+  R* P = Ps + g * NBINS;
   const float* x = samples + (size_t)row * N;
-  const long long s0 = (long long)f * hop - NFFT / 2;  // center=True
+  const long long s0 = (long long)f * hop - (VGG ? 0 : NFFT / 2);  // center=True, except VGGish's framing
   for (int m = lt; m < NH; m += TPF) {
-    float a = 0.f, c = 0.f;
+    R a = 0, c = 0;
     if (live) {
       long long s = s0 + 2 * m, s1 = s0 + 2 * m + 1;
-      if (DB) {  // zero padding (pad_mode="constant"), any N
+      if (VGG) {  // the whole frame lies in the row (F is at most 1 + (N - 400) / hop); the window is 0 past 400
+        a = s < N ? (R)x[s] : R(0);
+        c = s1 < N ? (R)x[s1] : R(0);
+      } else if (DB) {  // zero padding (pad_mode="constant"), any N
         a = (s >= 0 && s < N) ? x[s] : 0.f;
         c = (s1 >= 0 && s1 < N) ? x[s1] : 0.f;
       } else {  // reflect padding: N > NFFT / 2, so one reflection reaches
@@ -70,24 +78,29 @@ __global__ void __launch_bounds__(THREADS) mel_spec_kernel(const float* __restri
       a *= t.fft.window[2 * m];
       c *= t.fft.window[2 * m + 1];
     }
-    z[__brev(m) >> (32 - ilog2(NH))] = make_float2(a, c);
+    z[__brev(m) >> (32 - ilog2(NH))] = C2{a, c};
   }
   __syncthreads();
   fft_radix2<NFFT>(z, t.fft.twiddle, lt, TPF);
   for (int k = lt; k < NBINS; k += TPF) {
-    const float2 X = rfft_bin<NFFT>(z, t.fft.twiddle, k);
-    const float p = X.x * X.x + X.y * X.y;
-    P[k] = DB ? p : sqrtf(p);
+    const C2 X = rfft_bin<NFFT>(z, t.fft.twiddle, k);
+    const R p = X.x * X.x + X.y * X.y;
+    P[k] = DB ? p : VGG ? (R)sqrt((double)p) : (R)sqrtf((float)p);
   }
   __syncthreads();
   if (!live) return;
-  const int n_mels = DB ? ONSET_NMELS : t.n_mels;
+  const int n_mels = DB ? ONSET_NMELS : VGG ? VGGISH_NMELS : t.n_mels;
   for (int m = lt; m < n_mels; m += TPF) {
     const int o0 = t.bank.off[m], o1 = t.bank.off[m + 1];
-    const float* p = P + t.bank.lo[m] - o0;
-    float s = 0.f;
-    for (int o = o0; o < o1; ++o) s = fmaf(t.bank.w[o], p[o], s);
-    if (DB)
+    const R* p = P + t.bank.lo[m] - o0;
+    R s = 0;
+    for (int o = o0; o < o1; ++o) {
+      if (VGG) s = (R)fma((double)t.bank.w[o], (double)p[o], (double)s);
+      else s = (R)fmaf((float)t.bank.w[o], (float)p[o], (float)s);
+    }
+    if (VGG)
+      out[((size_t)row * F + f) * VGGISH_NMELS + m] = (float)log(s + 0.01);
+    else if (DB)
       out[((size_t)row * F + f) * ONSET_NMELS + m] = 10.f * log10f(fmaxf(1e-10f, s));
     else
       out[((size_t)row * n_mels + m) * F + f] = s;
@@ -160,7 +173,7 @@ double mel_to_hz(double m) {
   return m >= min_log_mel ? min_log_hz * std::exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
-cudaError_t spec_args(int sr, const vnb_mel_scale& s, MelSpecArgs* t) {
+cudaError_t spec_args(int sr, const vnb_mel_scale& s, MelSpecArgs<float>* t) {
   cudaError_t e = fft_tables(s.n_fft, &t->fft);
   if (e != cudaSuccess) return e;
   t->n_mels = s.n_mels;
@@ -235,10 +248,11 @@ cudaError_t mel_filterbank(int sr, int n_fft, int n_mels, double fmin, double fm
 cudaError_t launch_spectrogram(SpecMode mode, const float* samples, int rows, int N, int hop, int n_fft,
                                const FftTables& fft, const MelBank& bank, int n_mels, float* out, cudaStream_t st) {
   const int F = 1 + N / hop;
-  const MelSpecArgs t{fft, bank, n_mels};
+  const MelSpecArgs<float> t{fft, bank, n_mels};
 #define SPEC_LAUNCH(NF, MODE)                                                                                    \
   mel_spec_kernel<NF, MODE><<<dim3((F + MelGeom<NF>::FPC - 1) / MelGeom<NF>::FPC, rows), THREADS, 0, st>>>(      \
       samples, N, F, hop, t, out)
+  if (mode == SpecMode::VGGISH_LOG) return cudaErrorInvalidValue;  // launch_vggish_frontend: float64 tables
   if (mode == SpecMode::ONSET_DB) {
     if (n_fft != ONSET_NFFT || n_mels != ONSET_NMELS) return cudaErrorInvalidValue;
     SPEC_LAUNCH(ONSET_NFFT, SpecMode::ONSET_DB);
@@ -251,6 +265,80 @@ cudaError_t launch_spectrogram(SpecMode mode, const float* samples, int rows, in
     }
   }
 #undef SPEC_LAUNCH
+  count_launch();
+  return cudaGetLastError();
+}
+
+// VGGish's tables, in float64 (vggish_input.py / mel_features.py): the 512-point twiddles and the periodic Hann window
+// of length 400 zero-extended to 512 (one table), and spectrogram_to_mel_matrix(64, 257, 16000, 125, 7500): HTK mel
+// 1127 ln(1 + f / 700), triangles in mel space over linspace(0, 8000, 257), DC row zeroed, no normalisation.  Their
+// keys carry the table kind, so they cannot collide with the fp32 FFT tables and Slaney banks.
+static cudaError_t vggish_tables(FftTablesT<double>* fft, MelBankT<double>* bank) {
+  constexpr int NBINS = VGGISH_NFFT / 2 + 1;
+  const size_t b_tw = sizeof(double2) * NBINS;
+  const char* p = nullptr;
+  cudaError_t e = device_table({TABLE_VGGISH_FFT, (double)VGGISH_NFFT, (double)VGGISH_WIN}, [&] {
+    std::vector<char> img(b_tw + sizeof(double) * VGGISH_NFFT);
+    double2* tw = reinterpret_cast<double2*>(img.data());
+    double* win = reinterpret_cast<double*>(img.data() + b_tw);
+    for (int k = 0; k < NBINS; ++k) {
+      const double a = 2.0 * M_PI * k / VGGISH_NFFT;
+      tw[k] = make_double2(std::cos(a), -std::sin(a));
+    }
+    for (int k = 0; k < VGGISH_NFFT; ++k) win[k] = k < VGGISH_WIN ? 0.5 - 0.5 * std::cos(2.0 * M_PI * k / VGGISH_WIN) : 0.0;
+    return img;
+  }, &p);
+  if (e != cudaSuccess) return e;
+  fft->twiddle = reinterpret_cast<const double2*>(p);
+  fft->window = reinterpret_cast<const double*>(p + b_tw);
+  // off, lo, then the float64 weights, each at a 256-byte aligned offset (the doubles need 8-byte alignment)
+  size_t o = 0;
+  const size_t at_off = carve(o, sizeof(int32_t) * (VGGISH_NMELS + 1)), at_lo = carve(o, sizeof(int32_t) * VGGISH_NMELS);
+  const size_t at_w = o;
+  e = device_table({TABLE_VGGISH_HTK, (double)VGGISH_SR, (double)VGGISH_NFFT, (double)VGGISH_NMELS, VGGISH_FMIN,
+                    VGGISH_FMAX}, [&] {
+    auto mel = [](double f) { return 1127.0 * std::log(1.0 + f / 700.0); };
+    const double m0 = mel(VGGISH_FMIN), m1 = mel(VGGISH_FMAX), step = (m1 - m0) / (VGGISH_NMELS + 1);
+    std::vector<double> edges(VGGISH_NMELS + 2), bins(NBINS), wpack;
+    for (int i = 0; i < VGGISH_NMELS + 2; ++i) edges[i] = i == VGGISH_NMELS + 1 ? m1 : m0 + i * step;  // np.linspace
+    for (int k = 0; k < NBINS; ++k) bins[k] = mel(k * ((VGGISH_SR / 2.0) / (NBINS - 1)));
+    std::vector<int32_t> off(VGGISH_NMELS + 1), lo(VGGISH_NMELS);
+    std::vector<double> row(NBINS);
+    for (int m = 0; m < VGGISH_NMELS; ++m) {
+      int first = -1, last = -1;
+      for (int k = 0; k < NBINS; ++k) {
+        const double lower = (bins[k] - edges[m]) / (edges[m + 1] - edges[m]);
+        const double upper = (edges[m + 2] - bins[k]) / (edges[m + 2] - edges[m + 1]);
+        row[k] = k == 0 ? 0.0 : std::max(0.0, std::min(lower, upper));
+        if (row[k] != 0.0) { if (first < 0) first = k; last = k; }
+      }
+      off[m] = (int32_t)wpack.size();
+      lo[m] = first < 0 ? 0 : first;
+      if (first >= 0) wpack.insert(wpack.end(), row.begin() + first, row.begin() + last + 1);
+    }
+    off[VGGISH_NMELS] = (int32_t)wpack.size();
+    std::vector<char> img(at_w + sizeof(double) * wpack.size());
+    memcpy(img.data() + at_off, off.data(), sizeof(int32_t) * off.size());
+    memcpy(img.data() + at_lo, lo.data(), sizeof(int32_t) * lo.size());
+    if (!wpack.empty()) memcpy(img.data() + at_w, wpack.data(), sizeof(double) * wpack.size());
+    return img;
+  }, &p);
+  if (e != cudaSuccess) return e;
+  bank->off = reinterpret_cast<const int32_t*>(p + at_off);
+  bank->lo = reinterpret_cast<const int32_t*>(p + at_lo);
+  bank->w = reinterpret_cast<const double*>(p + at_w);
+  return cudaSuccess;
+}
+
+cudaError_t launch_vggish_frontend(const float* samples, int rows, int N, float* out, cudaStream_t st) {
+  MelSpecArgs<double> t;
+  t.n_mels = VGGISH_NMELS;
+  cudaError_t e = vggish_tables(&t.fft, &t.bank);
+  if (e != cudaSuccess) return e;
+  const int F = vggish_examples(N) * VGGISH_EX_FRAMES;
+  constexpr int FPC = MelGeom<VGGISH_NFFT>::FPC;
+  mel_spec_kernel<VGGISH_NFFT, SpecMode::VGGISH_LOG><<<dim3((F + FPC - 1) / FPC, rows), THREADS, 0, st>>>(
+      samples, N, F, VGGISH_HOP, t, out);
   count_launch();
   return cudaGetLastError();
 }
@@ -282,7 +370,7 @@ MelLossPlan mel_loss_plan(int B, int C, int N, int sr, const vnb_mel_scale* scal
 
 cudaError_t launch_mel_spectrogram(const float* samples, int rows, int N, int sr, const vnb_mel_scale& s, float* out,
                                    cudaStream_t st) {
-  MelSpecArgs t;
+  MelSpecArgs<float> t;
   cudaError_t e = spec_args(sr, s, &t);
   if (e != cudaSuccess) return e;
   return launch_spectrogram(SpecMode::MEL_MAG, samples, rows, N, s.hop, s.n_fft, t.fft, t.bank, t.n_mels, out, st);
@@ -301,7 +389,7 @@ cudaError_t launch_mel_loss(const float* x, const float* y, const MelLossPlan& p
   for (int i = 0; i < p.n_scales; ++i) {
     const MelScalePlan& s = p.s[i];
     const vnb_mel_scale sc{s.n_fft, s.hop, s.n_mels, s.fmin, s.fmax};
-    MelSpecArgs t;
+    MelSpecArgs<float> t;
     cudaError_t e = spec_args(p.sr, sc, &t);
     if (e != cudaSuccess) return e;
     if ((e = launch_spectrogram(SpecMode::MEL_MAG, x, rows, p.N, s.hop, s.n_fft, t.fft, t.bank, t.n_mels, X, st)))

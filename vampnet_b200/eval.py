@@ -1,12 +1,14 @@
 """Score an experiment directory's conditions against its baseline by multi-scale mel distance, on the GPU:
 
-    python -m vampnet_b200.eval --exp_dir D [--baseline_key baseline] [--audio_ext .wav]
+    python -m vampnet_b200.eval --exp_dir D [--baseline_key baseline] [--audio_ext .wav] [--vggish_ckpt PATH]
 
-The reference's scripts/exp/eval.py restated without FAD (DESIGN.md §13).  D holds one directory of audio files per
+The reference's scripts/exp/eval.py restated (DESIGN.md §13, §14).  D holds one directory of audio files per
 condition, named by integer stems (0.wav, 1.wav, ...), as the reference's scripts/exp/experiment.py writes them.  Every
 condition other than the baseline is scored file by file against the baseline with MelSpectrogramLoss(), and two CSV
 files are written into D: metrics-all.csv (mel,condition,file) and stats-mel.csv (condition,mean,count,std, std with
-ddof 1).
+ddof 1).  With --vggish_ckpt (torchvggish's checkpoint), each condition directory is also scored against the baseline
+directory by Fréchet audio distance (vampnet_b200.fad, every file of both directories), metrics-all.csv gets the column
+(mel,frechet,condition,file) and stats-frechet.csv is written the same way.
 """
 from __future__ import annotations
 
@@ -60,15 +62,29 @@ def _load_pair(cond: str, base_file: Path, cond_file: Path):
     return base, sig
 
 
-def evaluate(exp_dir, baseline_key: str = "baseline", audio_ext: str = ".wav", loss=None):
+def _write_stats(path, rows, col):
+    with open(path, "w", newline="") as f:
+        w = csv.writer(f)
+        w.writerow(["condition", "mean", "count", "std"])
+        for cond in sorted({r[-2] for r in rows}):
+            v = np.array([r[col] for r in rows if r[-2] == cond], dtype=np.float64)
+            std = float(np.std(v, ddof=1)) if v.size > 1 else math.nan
+            w.writerow([cond, repr(float(v.mean())), v.size, "" if math.isnan(std) else repr(std)])
+
+
+def evaluate(exp_dir, baseline_key: str = "baseline", audio_ext: str = ".wav", loss=None, fad=None):
     """Scores every condition; returns the rows of metrics-all.csv as (mel, condition, file) and writes both CSVs.
     loss(x, y) takes two batched AudioSignals and returns one value per item; the default is
-    MelSpectrogramLoss().per_item.  The pairs of one condition that share a shape and rate are scored in one call."""
+    MelSpectrogramLoss().per_item.  The pairs of one condition that share a shape and rate are scored in one call.
+    With fad (a vampnet_b200.fad.FrechetAudioDistance) the rows are (mel, frechet, condition, file), frechet the
+    distance between the condition's directory and the baseline's (whose embeddings are computed once), and
+    stats-frechet.csv is written too."""
     exp_dir = Path(exp_dir)
     if loss is None:
         from .metrics import MelSpectrogramLoss
         loss = MelSpectrogramLoss().per_item
     rows = []
+    base_moments = fad.dir_moments(exp_dir / baseline_key, audio_ext) if fad is not None else None
     for cond, pairs in _pairs(exp_dir, baseline_key, audio_ext):
         loaded = [_load_pair(cond, b, c) for b, c in pairs]
         groups = {}
@@ -83,18 +99,18 @@ def evaluate(exp_dir, baseline_key: str = "baseline", audio_ext: str = ".wav", l
             y = AudioSignal(torch.cat([loaded[i][1].audio_data for i in idx]), sr)
             for i, v in zip(idx, torch.as_tensor(loss(x, y)).reshape(-1).tolist()):
                 mel[i] = float(v)
-        rows.extend((mel[i], cond, pairs[i][0].stem) for i in range(len(loaded)))
+        if fad is None:
+            rows.extend((mel[i], cond, pairs[i][0].stem) for i in range(len(loaded)))
+        else:
+            frechet = fad.score_moments(base_moments, fad.dir_moments(exp_dir / cond, audio_ext))
+            rows.extend((mel[i], frechet, cond, pairs[i][0].stem) for i in range(len(loaded)))
     with open(exp_dir / "metrics-all.csv", "w", newline="") as f:
         w = csv.writer(f)
-        w.writerow(["mel", "condition", "file"])
-        w.writerows([repr(m), c, s] for m, c, s in rows)
-    with open(exp_dir / "stats-mel.csv", "w", newline="") as f:
-        w = csv.writer(f)
-        w.writerow(["condition", "mean", "count", "std"])
-        for cond in sorted({c for _, c, _ in rows}):
-            v = np.array([m for m, c, _ in rows if c == cond], dtype=np.float64)
-            std = float(np.std(v, ddof=1)) if v.size > 1 else math.nan
-            w.writerow([cond, repr(float(v.mean())), v.size, "" if math.isnan(std) else repr(std)])
+        w.writerow(["mel", "condition", "file"] if fad is None else ["mel", "frechet", "condition", "file"])
+        w.writerows([repr(v) for v in r[:-2]] + list(r[-2:]) for r in rows)
+    _write_stats(exp_dir / "stats-mel.csv", rows, 0)
+    if fad is not None:
+        _write_stats(exp_dir / "stats-frechet.csv", rows, 1)
     return rows
 
 
@@ -103,10 +119,16 @@ def main(argv=None):
     ap.add_argument("--exp_dir", required=True)
     ap.add_argument("--baseline_key", default="baseline")
     ap.add_argument("--audio_ext", default=".wav")
+    ap.add_argument("--vggish_ckpt", default=None, help="torchvggish checkpoint: also score by Fréchet audio distance")
     a = ap.parse_args(argv)
-    rows = evaluate(a.exp_dir, a.baseline_key, a.audio_ext)
-    print(f"scored {len(rows)} files in {len({c for _, c, _ in rows})} conditions; wrote "
-          f"{Path(a.exp_dir) / 'metrics-all.csv'} and {Path(a.exp_dir) / 'stats-mel.csv'}")
+    fad = None
+    if a.vggish_ckpt is not None:
+        from .fad import FrechetAudioDistance
+        fad = FrechetAudioDistance(a.vggish_ckpt, use_pca=False, use_activation=False)
+    rows = evaluate(a.exp_dir, a.baseline_key, a.audio_ext, fad=fad)
+    d = Path(a.exp_dir)
+    stats = f"{d / 'stats-mel.csv'}" + ("" if fad is None else f" and {d / 'stats-frechet.csv'}")
+    print(f"scored {len(rows)} files in {len({r[-2] for r in rows})} conditions; wrote {d / 'metrics-all.csv'} and {stats}")
 
 
 if __name__ == "__main__":
