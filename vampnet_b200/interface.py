@@ -424,7 +424,6 @@ class Interface(torch.nn.Module):
 
         mixed_top_p=True: chunks of nucleus (top-p) and plain-sampling requests share launches too
         (generate_many(mixed_top_p=True) in both stages); the results are the same."""
-        from .modules.transformer import draw_philox_key
         many = dict(mixed_lengths=True) if mixed_lengths else {}
         if mixed_steps:
             many["mixed_steps"] = True
@@ -433,24 +432,42 @@ class Interface(torch.nn.Module):
         reqs = []
         for r in requests:
             r = dict(r)
-            q = dict(codes=r.pop("codes"), mask=r.pop("mask"), batch_size=r.pop("batch_size", 1),
-                      feedback_steps=r.pop("feedback_steps", 1), time_stretch_factor=r.pop("time_stretch_factor", 1),
-                      return_mask=r.pop("return_mask", False))
-            q["z"], q["mask"] = self._vamp_inputs(q["codes"], q["mask"], q["batch_size"], q["time_stretch_factor"])
-            q["zv"] = q["z"]
+            codes, mask, batch_size = r.pop("codes"), r.pop("mask"), r.pop("batch_size", 1)
+            feedback_steps, k = r.pop("feedback_steps", 1), r.pop("time_stretch_factor", 1)
+            return_mask = r.pop("return_mask", False)
+            z, mask = self._vamp_inputs(codes, mask, batch_size, k)
             seed, key = r.pop("seed", None), r.pop("philox_key", None)
             adapter = r.pop("adapter", None)
-            q["with_adapter"] = {} if adapter is None else dict(adapter=adapter)
-            q["gen"] = dict(r, **q["with_adapter"])
-
-            def keys(n, seed=seed, key=key):
-                return [key if key is not None else draw_philox_key(seed) for _ in range(n)]
-            # what the sequential vamp() draws: each coarse pass's chunks, then the fine stage's chunks
-            n_frames = q["z"].shape[-1]
-            n_coarse = len(self._spans(n_frames, self.s2t(self.coarse.chunk_size_s)))
-            q["keys"] = [keys(n_coarse) for _ in range(q["feedback_steps"])]
-            q["c2f_keys"] = [draw_philox_key(None) for _ in self._spans(n_frames, self.s2t(self.c2f.chunk_size_s))]
+            with_adapter = {} if adapter is None else dict(adapter=adapter)
+            q = self._vamp_request(z, mask, feedback_steps, dict(r, **with_adapter),
+                                   fine=dict(self._C2F_KWARGS, **with_adapter), fine_mask=mask, seed=seed, key=key)
+            q["return_mask"] = return_mask
             reqs.append(q)
+        self._run_vamp_requests(reqs, many)
+        return [self._vamp_result(q["z"], q["zv"], q.get("coarse_start"), q["fine_start"], q["return_mask"])
+                for q in reqs]
+
+    def _vamp_request(self, z, mask, feedback_steps: int, gen: dict, fine: dict = None, fine_mask=None, seed=None,
+                      key=None) -> dict:
+        """A request for _run_vamp_requests, with the Philox keys of all its generate calls drawn now, in the order the
+        sequential calls draw them: `feedback_steps` coarse_vamp passes over codes z with `mask` and generate keyword
+        arguments `gen` (0 passes: no coarse stage; seed / key as generate's seed / philox_key), then, unless fine is
+        None, coarse_to_fine of the result with generate keyword arguments `fine` and mask fine_mask."""
+        from .modules.transformer import draw_philox_key
+        n_frames = z.shape[-1]
+        n_coarse = len(self._spans(n_frames, self.s2t(self.coarse.chunk_size_s)))
+        keys = [[key if key is not None else draw_philox_key(seed) for _ in range(n_coarse)]
+                for _ in range(feedback_steps)]
+        c2f_keys = [] if fine is None else [draw_philox_key(None)
+                                            for _ in self._spans(n_frames, self.s2t(self.c2f.chunk_size_s))]
+        return dict(z=z, mask=mask, zv=z, feedback_steps=feedback_steps, gen=gen, keys=keys, fine=fine,
+                    fine_mask=fine_mask, c2f_keys=c2f_keys)
+
+    def _run_vamp_requests(self, reqs: list, many: dict):
+        """Run prepared requests (_vamp_request) stage by stage: coarse pass i of every request that has one as one
+        coarse generate_many(**many), then the fine stage of every request that has one as one c2f generate_many.  Sets
+        each request's "zv" (its result), "coarse_start" and "fine_start" (the masked inputs of its last coarse pass and
+        of its fine stage, where it has them and a fine_mask)."""
         for i in range(max((q["feedback_steps"] for q in reqs), default=0)):
             stage = [q for q in reqs if q["feedback_steps"] > i]
             plans = [self._coarse_plan(q["zv"], q["mask"]) for q in stage]
@@ -460,12 +477,13 @@ class Interface(torch.nn.Module):
             for q, plan in zip(stage, plans):
                 q["zv"], start = self._coarse_stitch(q["zv"], plan, [next(results) for _ in plan], True)
                 q["coarse_start"] = start.roll(shifts=(i + 1) % q["feedback_steps"], dims=-1)
-        plans = [self._c2f_plan(self._with_fine_books(q["z"], q["zv"]), q["mask"]) for q in reqs]
-        calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **self._C2F_KWARGS, **q["with_adapter"])
-                 for q, (chunks, _) in zip(reqs, plans) for c, k in zip(chunks, q["c2f_keys"])]
+        stage = [q for q in reqs if q["fine"] is not None]
+        if not stage:
+            return
+        plans = [self._c2f_plan(self._with_fine_books(q["z"], q["zv"]), q["fine_mask"]) for q in stage]
+        calls = [dict(**c, return_signal=False, cfg_guidance=None, philox_key=k, **q["fine"])
+                 for q, (chunks, _) in zip(stage, plans) for c, k in zip(chunks, q["c2f_keys"])]
         results = iter(self.c2f.generate_many(self.codec, calls, **many))
-        out = []
-        for q, (chunks, state) in zip(reqs, plans):
-            zv, fine_start = self._c2f_stitch([next(results) for _ in chunks], state, True)
-            out.append(self._vamp_result(q["z"], zv, q.get("coarse_start"), fine_start, q["return_mask"]))
-        return out
+        for q, (chunks, state) in zip(stage, plans):
+            out = self._c2f_stitch([next(results) for _ in chunks], state, q["fine_mask"] is not None)
+            q["zv"], q["fine_start"] = out if q["fine_mask"] is not None else (out, None)
